@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — graphs/sec through the message-passing hot path, forward + backward (BASELINE.json metric).
 
-    python bench.py [--config NAME] [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--config NAME] [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
 
 --config picks the BASELINE.json configuration (default `masking`, the one the metric is quoted on):
 
@@ -21,6 +21,12 @@ one D2H read of the loss per step (issued asynchronously after the step, consume
 `loss_accum += loss.item()` only feeds a log line).  L2 is flushed between timed steps (256 MiB memset outside the per-step
 event pairs).  `--impl reference` times the reference's OWN model.py on the host cores (oracle/reference_runner.py;
 kind "reference"), or the oracle port of it when the reference's sources are not on the box (kind "port").
+
+`--dump-outputs DIR` writes what the last step of the device-resident timed pass (the one `value` is quoted on; the e2e pass
+is not dumped) returned to its caller: `loss.npy` (float64) and one `grad.<parameter>.npy` (float32) per parameter, at most
+64 MiB in all (beyond that every array is cut to a fixed, seeded sample of its elements, `<name>.idx.npy` holding the int64
+flat indices, both counted in the 64 MiB).  Batches and initial parameters are seeded, so two
+builds run with the same arguments can be compared output for output.
 """
 import argparse
 import gc
@@ -69,17 +75,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tensor=d["bf16_tflops"], tensor_sustained=d.get("bf16_tflops_sustained"), src="measured")
-    return dict(hbm=6650.0, tensor=1590.0, tensor_sustained=1400.0, src="fallback")
-
-
-def measured_traffic():
-    """DRAM bytes per launch of the two roofline kernels from this round's `ncu --set full` captures: profiles/traffic.json,
-    written by tools/ncu_traffic.py from the committed capture (never a constant typed into this file)."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        return json.load(open(p))
-    except Exception:
-        return {}
+    # NVIDIA H100 SXM data sheet (700 W board): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16; not measured here
+    return dict(hbm=3350.0, tensor=989.0, tensor_sustained=None, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -306,8 +303,34 @@ def work_model(config, b):
 
 
 # ---------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ---------------------------------------------------------------------------------------------------
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(d, loss, named_grads):
+    """Write the arrays a caller of the step receives (see the module docstring)."""
+    import numpy as np
+    arrays = {"loss": loss.detach().double().cpu().reshape(-1).numpy()}
+    for k, g in named_grads:
+        if g is not None:
+            arrays["grad." + k] = g.detach().float().cpu().numpy()
+    total = sum(a.nbytes for a in arrays.values())
+    os.makedirs(d, exist_ok=True)
+    rng = np.random.default_rng(0)
+    # a kept element costs its value plus an int64 index; every array keeps the same fraction, and 256 bytes per file
+    # are set aside for the .npy headers
+    budget = DUMP_BYTES - 2 * 256 * len(arrays)
+    sampled_bytes = sum(a.size * (a.itemsize + 8) for a in arrays.values())
+    for k, a in arrays.items():
+        if total > DUMP_BYTES and a.size > 1:
+            keep = max(1, a.size * budget // sampled_bytes)
+            idx = np.sort(rng.choice(a.size, size=keep, replace=False)).astype(np.int64)
+            np.save(os.path.join(d, k + ".idx.npy"), idx)
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(d, k + ".npy"), a)
+
+
 def run_b200(args, rank, world, local_rank):
     import torch.distributed as dist
     ts = importlib.import_module("pretrain-gnns_b200.train_steps")
@@ -396,7 +419,7 @@ def run_b200(args, rank, world, local_rank):
                     loss_ready[j].synchronize()
                     acc += float(loss_host[j])
             else:
-                train_step(resident[i % len(resident)])
+                loss = train_step(resident[i % len(resident)])
             ev[i][1].record()
         if e2e:
             for i in range(max(args.steps - LAG, 0), args.steps):
@@ -410,6 +433,7 @@ def run_b200(args, rank, world, local_rank):
         per = [a.elapsed_time(b) for a, b in ev]
         host_t.append(t0 + wall)
         timed.host_issue_ms = [1e3 * (b - a) for a, b in zip(host_t[:-1], host_t[1:])]  # host time per loop iteration (diagnostic)
+        timed.last_loss = loss if args.steps > 0 else None
         t = torch.tensor([sum(per)], dtype=torch.float64, device=dev)
         if world > 1:
             # every rank's own figures (sum, slowest step and its index), so that a slow rank can be told from a slow step
@@ -425,6 +449,8 @@ def run_b200(args, rank, world, local_rank):
 
     with ClockSampler(local_rank) as clocks:
         ms_dev, launches, wall_dev, per_dev, _ = timed(False)
+        if args.dump_outputs and rank == 0 and args.steps > 0:   # before anything else runs a step and overwrites the gradients
+            dump_outputs(args.dump_outputs, timed.last_loss, step.named_parameters())
         host_dev = timed.host_issue_ms
         per_rank_dev = timed.per_rank
         ms_e2e, _, wall_e2e, per_e2e, mean_loss = timed(True)
@@ -454,7 +480,7 @@ def run_b200(args, rank, world, local_rank):
         "vs_baseline": None, "dtype": "f32" if ops.get_precision() == "fp32" else "tf32x3", "data": "synthetic",
         "config": cfg,
         "detail": {"nodes_per_batch": wm["nodes"], "edges_per_batch": wm["edges"], "distinct_batches": NUM_DISTINCT_BATCHES,
-                   "gemm_precision": ops.get_precision() + (" (error-compensated 3xTF32 on tcgen05, fp32-class: measured 1-3e-6 of scale; "
+                   "gemm_precision": ops.get_precision() + (" (error-compensated 3xTF32 on wgmma, fp32-class; "
                                                             "--precision fp32 runs the exact FFMA kernels)" if ops.get_precision() != "fp32" else ""),
                    "grad_allreduce": (reducer.backend if reducer is not None else "none (1 GPU)"),
                    "per_step_ms": dist_stats(per_dev), "per_step_ms_e2e": dist_stats(per_e2e),
@@ -522,7 +548,7 @@ def in_step_rooflines(cabi, train_step, resident, flush, roof, roof_gather, wm, 
     fam = wm["gemm_flops_per_step"] / (gemm_us / steps * 1e-6) / 1e12 if gemm_us else None
     roof["isolated"] = {"achieved": roof["achieved"], "frac": roof["frac"], "us_per_launch": roof["us_per_launch"], "kernel": roof["kernel"]}
     if fam is not None:
-        roof.update(kernel="tcgen05 3xTF32 GEMM family of the step (fwd + dgrad + split-K wgrad of every Linear): total algorithmic "
+        roof.update(kernel="wgmma 3xTF32 GEMM family of the step (fwd + dgrad + split-K wgrad of every Linear): total algorithmic "
                            "flops / total in-step kernel time", achieved=fam, frac=fam / roof["peak"], us_per_step=gemm_us / steps,
                     share_of_step=gemm_us / total,
                     timing="sum over %d training steps of every GEMM launch's CUDA-event duration (library timing mode)" % steps,
@@ -551,7 +577,6 @@ def kernel_rooflines(ops, config, b, dev, wm):
     """Isolated timings (CUDA events on the launch stream, L2 flushed before each launch) of the two kernels the step is made
     of: the config's largest forward GEMM (tensor-bound) and its neighbour gather (HBM/L2-bound)."""
     pk = peaks()
-    tr = measured_traffic()
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     if config == "contextpred":
         x_key, ei_key, ea_key = "x_substruct", "edge_index_substruct", "edge_attr_substruct"
@@ -594,17 +619,13 @@ def kernel_rooflines(ops, config, b, dev, wm):
     ach = gflop / (t_gemm * 1e-3) / 1e12
     roof = {"bound": "tensor", "kernel": "largest forward Linear of the step [%d,%d]x[%d,%d] + bias + ReLU (%s)" % (M, K, K, N, mode),
             "achieved": ach, "peak": pk["tensor"], "unit": "TFLOP/s", "frac": ach / pk["tensor"],
-            "traffic": tr.get(config, {}).get("gemm", {}).get("dram_bytes_per_launch"),
-            "traffic_source": tr.get(config, {}).get("gemm", {}).get("source"),
-            "peak_source": pk["src"] + " cuBLAS bf16 dense burst (MEASURED_PEAKS.json)",
+            "peak_source": pk["src"] + (" cuBLAS bf16 dense burst (MEASURED_PEAKS.json)" if pk["src"] == "measured" else ""),
             "note": "fp32-equivalent flops; ceiling of the 3xTF32 scheme = peak/6 = %.0f TFLOP/s (achieved/ceiling = %.3f)"
                     % (pk["tensor"] / 6, ach / (pk["tensor"] / 6)),
             "us_per_launch": t_gemm * 1e3}
     roof_g = {"bound": "hbm", "kernel": "%s (gather + segment reduce, one layer pass)" % wm["gather_kernel"],
               "achieved": gbytes / (t_gather * 1e-3) / 1e9, "peak": pk["hbm"], "unit": "GB/s",
               "frac": gbytes / (t_gather * 1e-3) / 1e9 / pk["hbm"],
-              "traffic": tr.get(config, {}).get("gather", {}).get("dram_bytes_per_launch"),
-              "traffic_source": tr.get(config, {}).get("gather", {}).get("source"),
               "peak_source": pk["src"], "us_per_launch": t_gather * 1e3, "algorithmic_bytes": gbytes}
     return roof, roof_g
 
@@ -618,6 +639,7 @@ def main():
     ap.add_argument("--config", default="masking", choices=CONFIG_NAMES)
     ap.add_argument("--precision", default=None, choices=[None, "fp32", "tf32x3"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the loss and gradients of the last device-resident timed step as DIR/<name>.npy (<= 64 MiB)")
     args = ap.parse_args()
     if args.steps is None:
         args.steps = 20 if args.config == "bio_supervised" else 50

@@ -1,5 +1,5 @@
 /*
- * pgnn_b200.h — C ABI of libpgnn_b200.so: the B200 (sm_100a) message-passing hot path of
+ * pgnn_b200.h — C ABI of libpgnn_b200.so: the H100 (sm_90a) message-passing hot path of
  * snap-stanford/pretrain-gnns (chem/model.py, bio/model.py).
  *
  * The reference exposes NO native interface for this path: its arithmetic runs inside
@@ -146,7 +146,7 @@ PGNN_API int pgnn_edge_table_bwd(const float* S, int64_t Q, const float* g, int6
 /* ---------------------------------------------------------------------------------------------
  * Dense node transforms (torch.nn.Linear inside GINConv.mlp chem/model.py:29, bio/model.py:24;
  * GCN/SAGE/GAT linear chem/model.py:99,147,194).  precision: 0 = fp32 FFMA (SIMT),
- * 1 = 3xTF32 error-compensated tcgen05 (falls back to 0 where a shape is unsupported).
+ * 1 = 3xTF32 error-compensated wgmma (falls back to 0 where a shape is unsupported).
  * ------------------------------------------------------------------------------------------- */
 /* y[M,N] = act(x[M,K] . w[N,K]^T + bias[N]) ; relu != 0 applies max(.,0) */
 PGNN_API int pgnn_linear_fwd(const float* x, int64_t ldx, const float* w, const float* bias,

@@ -1,4 +1,4 @@
-"""Build libpgnn_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libpgnn_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python pretrain-gnns_b200/build.py [--force]
 
@@ -18,7 +18,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.environ.get("PGNN_BUILD_DIR") or os.path.join(HERE, "csrc", "_obj")
 LIB = os.environ.get("PGNN_LIB_OUT") or os.path.join(HERE, "libpgnn_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 

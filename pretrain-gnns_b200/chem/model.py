@@ -49,7 +49,7 @@ class _BondTables(nn.Module):
         try:
             return _AGGR_MODE[self.aggr]
         except KeyError:
-            raise ValueError("aggr=%r is not supported by the B200 path (add / mean only)" % (self.aggr,))
+            raise ValueError("aggr=%r is not supported by this path (add / mean only)" % (self.aggr,))
 
 
 class GINConv(_BondTables):
@@ -215,7 +215,7 @@ class GNN_graphpred(nn.Module):
         if graph_pooling == "mean":
             self.pool = global_mean_pool
         elif graph_pooling in ("sum", "max", "attention") or graph_pooling[:-1] == "set2set":
-            raise NotImplementedError("graph_pooling=%r is outside the B200 hot path (mean only)" % (graph_pooling,))
+            raise NotImplementedError("graph_pooling=%r is outside this hot path (mean only)" % (graph_pooling,))
         else:
             raise ValueError("Invalid graph pooling type.")
         self.mult = 1

@@ -1,4 +1,4 @@
-// Shared helpers for libpgnn_b200 (sm_100a only).
+// Shared helpers for libpgnn_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -79,8 +79,8 @@ struct PgnnBnFold {
 // per-column BatchNorm constants from the accumulated sums; `leader` performs the running-statistics side effects
 // Every CTA of the consumer runs this for its columns, so it must be cheap: the fp64 part is two multiplies and one FMA (the
 // sums are fp64 because E[x^2] - E[x]^2 cancels); the reciprocal square root is taken in fp32 like torch's own BatchNorm
-// kernels do.  (With fp64 division and square root — software sequences of ~100 instructions each — this prologue was most
-// of the 450 instructions per thread ncu counted in k_aggregate_fwd: profiles/r02_kernels_masking.md.)
+// kernels do.  (fp64 division and square root are software sequences of ~100 instructions each, which would dominate the
+// consumer kernel's prologue.)
 __device__ __forceinline__ void bn_fold_column(const PgnnBnFold& f, int C, int c, bool leader, float& scale, float& shift) {
   const double s = f.acc[c], ss = f.acc[(int64_t)C + c];
   const double mean = s * f.inv_m;
@@ -101,7 +101,7 @@ __device__ __forceinline__ void bn_fold_column(const PgnnBnFold& f, int C, int c
   }
 }
 
-// Epilogue of the tensor-core GEMM kernels (dense_tc.cu, dense_tma.cu)
+// Epilogue of the tensor-core GEMM kernel (dense_tc.cu)
 struct TcEpilogue {
   const float* bias;      // [N] or null
   int relu;
@@ -110,15 +110,10 @@ struct TcEpilogue {
   int atomic;             // split-K: accumulate with atomics into a zeroed output
   PgnnGemmHooks hooks;    // fused column reductions over the final output tile (not with split-K)
   int64_t split_stride = 0;  // split-K without atomics: split z stores its tile at C + z * split_stride (folded afterwards)
-  // In-kernel fold of those partial tiles (TMA kernel only; requires every CTA of the grid to be co-resident): after storing
-  // its partial tile a CTA bumps fold_counter[tile], waits until all `gridDim.z` splits of the tile have arrived, and sums a
-  // 1/gridDim.z row slice of the tile over the splits IN SPLIT ORDER (bit-reproducible) into fold_out (leading dimension ldc).
-  unsigned int* fold_counter = nullptr;  // [tiles], zero before the launch
-  float* fold_out = nullptr;
 };
 
-// B200: 148 SMs.  Grids for grid-stride kernels are sized as a multiple of this.
-constexpr int kNumSMs = 148;
+// H100 SXM: 132 SMs.  Grids for grid-stride kernels are sized as a multiple of this.
+constexpr int kNumSMs = 132;
 
 // Programmatic dependent launch (PDL).  Every kernel of this library starts with pdl_prologue(): wait until the
 // previous kernel in the stream has completed and flushed (griddepcontrol.wait), then allow the NEXT kernel's CTAs to
@@ -131,32 +126,6 @@ __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.lau
 __device__ __forceinline__ void pdl_prologue() {
   pdl_wait();
   pdl_trigger();
-}
-
-// same, for thread-block clusters of `cluster` CTAs along grid.x (kernels that use tcgen05 cta_group::2 are rejected with
-// cudaErrorInvalidClusterSize unless the pair lies along x)
-template <typename... KArgs, typename... Args>
-inline cudaError_t pgnn_launch_cluster_x(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, unsigned cluster,
-                                         Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  attr[1].id = cudaLaunchAttributeClusterDimension;
-  attr[1].val.clusterDim.x = cluster;
-  attr[1].val.clusterDim.y = 1;
-  attr[1].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 2;
-  const bool prof = g_pgnn_profile_on.load(std::memory_order_relaxed) != 0;
-  if (prof) pgnn_profile_mark(reinterpret_cast<const void*>(kernel), st, false);
-  const cudaError_t err = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
-  if (prof) pgnn_profile_mark(reinterpret_cast<const void*>(kernel), st, true);
-  return err;
 }
 
 template <typename... KArgs, typename... Args>

@@ -6,7 +6,7 @@
 //   dgrad  gx[M,K] = gy[M,N] . w[N,K]        A: reduction-contiguous   B: reduction-strided
 //   wgrad  gw[N,K] = gy[M,N]^T . x[M,K]      A: reduction-strided      B: reduction-strided  (split over rows)
 //
-// This is the exact-fp32 reference path of the library; the tensor-core path (3xTF32 tcgen05,
+// This is the exact-fp32 reference path of the library; the tensor-core path (3xTF32 wgmma,
 // dense_tc.cu) is checked against it.
 #include "common.cuh"
 
@@ -223,7 +223,7 @@ int pgnn_linear_bwd_w(const float* gy, int64_t ldgy, const float* x, int64_t ldx
     if (rc != PGNN_EUNSUPPORTED) return rc;
   }
   // gw[n, k] = sum_m gy[m, n] * x[m, k]: rows of the output are N, columns K, reduction over the M rows.
-  // Few output tiles (N*K is only 600x300), so split the row reduction until the grid covers the 148 SMs.
+  // Few output tiles (N*K is only 600x300), so split the row reduction until the grid covers the SMs twice.
   const int tiles = (int)(ceil_div(N, BM) * ceil_div(K, BN));
   int splits = (int)ceil_div(2 * kNumSMs, tiles);
   const int max_splits = (int)ceil_div(M, 4 * BK);

@@ -1,283 +1,383 @@
-// Dense node transforms on the 5th-generation tensor cores (precision 1): error-compensated 3xTF32.
+// Dense node transforms on the Hopper tensor cores (precision 1): error-compensated 3xTF32 with wgmma.
 //
-// fp32 parity (1e-4, north_star) rules out plain TF32 (10-bit mantissa over K = 300/600).  Every fp32
-// operand x is used as hi = the raw fp32 word (the tensor core reads its top 19 bits, i.e. truncates to
-// tf32) and lo = x - trunc_tf32(x) (exact in fp32); each k-step issues three tcgen05.mma (lo*hi, hi*lo,
-// hi*hi).  The dropped lo*lo term and the truncation of lo are ~2^-20 relative; measured GEMM error is
-// 1-3e-6 of the output scale, the same class as an fp32 FFMA GEMM (tools/check_tc.py).
+// fp32 parity (1e-4, north_star) rules out plain TF32 (10-bit mantissa over K = 300/600).  Every fp32 operand x
+// is split into hi = trunc_tf32(x) and lo = x - hi (exact in fp32); each k-step issues three wgmma (lo*hi, hi*lo,
+// hi*hi).  The dropped lo*lo term and the truncation of lo are ~2^-20 relative: the GEMM error is of the same class
+// as an fp32 FFMA GEMM (tools/check_tc.py).
 //
 // One kernel template serves the three operand layouts of dense.cu (same roles, same epilogues):
 //   fwd    y[M,N]  = x[M,K]  . w[N,K]^T      A K-major,  B K-major
 //   dgrad  gx[M,K] = gy[M,N] . w[N,K]        A K-major,  B MN-major (w rows are the reduction)
 //   wgrad  gw[N,K] = gy[M,N]^T . x[M,K]      A MN-major, B MN-major (node rows are the reduction; split-K)
 //
-// Structure (per CTA: one 128 x BN output tile; 8 producer warps + 1 MMA warp; 4 smem stages of BK = 16):
-//   * producers cp.async (16 B, L2-only, zero-filled out of bounds) the raw fp32 operand pieces straight into
-//     the UMMA canonical smem layouts (K-major: no-swizzle 8x16B core matrices; MN-major: 128B swizzle with
-//     32B base, the only layout tf32 accepts transposed), two blocks ahead; when a thread's own pieces of a
-//     block have landed (cp.async.wait_group) it re-reads them, writes lo into the stage's second buffer,
-//     fence.proxy.async's, and its warp arrives on full[stage];
-//   * the MMA warp waits full[stage], one lane issues 2 k-steps x 3 products and tcgen05.commit's onto
-//     empty[stage]; the hi*hi chain and the cross terms use separate TMEM accumulators (truncating adds);
-//   * epilogue (producer warps): tcgen05.ld both accumulators -> add -> bias / ReLU / mask -> global.
-// No block-wide barrier and no register-staged global load sits in the main loop: the only waits are
-// the two mbarrier rings and the thread's own cp.async group.
+// Structure (per CTA: one 128 x BN output tile, two warpgroups of 64 rows each, BK = 32 per block):
+//   * every thread loads its share of the next block (16-byte global loads along whichever extent is contiguous,
+//     zero-filled out of range) into registers while the tensor cores work on the current one;
+//   * it then splits the values into hi / lo and stores both into the other shared-memory stage in the
+//     K-major 128B-swizzled layout (tf32 wgmma reads K-major operands only, so MN-major sources are transposed
+//     on this store), and fences the stores to the async proxy;
+//   * per block and warpgroup: 4 k-steps x (BN / 64) column halves x 3 products of wgmma.m64n64k8; the hi*hi chain
+//     and the cross terms go to separate register accumulators;
+//   * epilogue: both accumulators are summed into a shared-memory staging tile, then written out row-contiguously
+//     with bias / ReLU / mask applied, plus the optional fused column reductions.
 #include <cstdlib>
 
-#include "tc_common.cuh"
+#include "common.cuh"
 
 namespace {
 
-constexpr int BK = 16;        // fp32 elements of the reduction per stage = 2 UMMA k-steps of 8
-constexpr int NTHREADS = NPRODUCER + 32;  // + one MMA-issuing warp
-// Rings: raw (= hi) operand stages filled by cp.async, and lo stages written by the producers just before a block
-// is published.  Measured: deeper raw rings / more groups in flight do not raise the block rate (one SM pulls
-// ~26 GB/s through LDGSTS whatever the depth) but lengthen the pipeline fill, so the rings stay balanced.
-constexpr int NRAW = 4;
-constexpr int NLO = 4;
-constexpr int AHEAD = 2;  // cp.async groups in flight per thread
+constexpr int BM = 128;        // rows per CTA: two warpgroups x wgmma M = 64
+constexpr int BK = 32;         // fp32 of the reduction per block = one 128-byte swizzle row
+constexpr int NTHREADS = 256;  // two warpgroups; every thread loads, converts, issues its warpgroup's wgmma and runs the epilogue
 
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// byte sizes of one operand buffer (hi or lo) for a tile of R rows (MN extent) x BK
-__host__ __device__ constexpr int kmajor_lbo(int R) { return R * 16 + 32; }          // stride between 16-byte k-chunks (+32: a quarter-warp = 2 rows x 4 chunks hits 8 distinct bank groups)
-__host__ __device__ constexpr int kmajor_bytes(int R) { return kmajor_lbo(R) * (BK / 4); }
-// MN-major tf32 operands must use the 128B-swizzle-with-32B-base layout (UMMA layout type 1): atoms of
-// [4 k][32 consecutive row indices] = 4 rows of 128 B, the 32-byte chunk index XOR-ed with (k mod 4).
-// A tile keeps the BK/4 atoms of one 32-row block contiguous: k-group stride (SBO) 512 B, block stride (LBO) 4 KiB.
-constexpr int MN_SBO = 512;
-constexpr int MN_LBO = (BK / 4) * MN_SBO;  // 2 KiB at BK = 16
-__host__ __device__ constexpr int mnmajor_bytes(int R) { return (R / 32) * MN_LBO; }
+// byte offset of element (r, k) in a K-major SWIZZLE_128B tile: 8-row groups of 1024 B, the 16-byte chunk index XOR-ed
+// with the row index mod 8
+__device__ __forceinline__ int sw128_off(int r, int k) { return (r >> 3) * 1024 + (r & 7) * 128 + ((((k >> 2) ^ (r & 7))) << 4) + (k & 3) * 4; }
 
-
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+// wgmma shared-memory matrix descriptor (sm_90): start >> 4 | LBO >> 4 << 16 (unused for swizzled K-major) | SBO >> 4 << 32 |
+// layout 1 (128B swizzle) << 62
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// Operand tile.  KC: source is contiguous along the reduction (element (r,k) at src[r*ld + k]); otherwise
-// contiguous along the row index (element (r,k) at src[k*ld + r]).  R = rows (MN extent) of the tile.
-// Each producer thread owns NV 16-byte pieces per block, the same ones in `issue` (cp.async raw -> smem) and in
-// `make_lo` (re-read own pieces, write x - trunc_tf32(x)).  Everything that does not depend on the block index
-// (global pointer of the piece in block 0, smem offset, row validity) is computed ONCE in `init`: the main
-// loop is a pointer bump, one compare and the cp.async per piece — with only two producer warps per scheduler
-// the per-block address arithmetic (div/mod by non-powers of two, 64-bit multiplies) was what bounded it.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// d[64 x 64] += a[64 x 8] . b[64 x 8]^T, tf32 operands from shared memory, fp32 accumulators in registers
+__device__ __forceinline__ void wgmma_tf32_m64n64k8(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db)
+      : "memory");
+}
+// keeps the compiler from moving accumulator registers across the asynchronous wgmma window
+__device__ __forceinline__ void fence_acc(float (&d)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+__device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
+
+// Operand tile loader.  KC: source contiguous along the reduction (element (r,k) at src[r*ld + k]); otherwise contiguous
+// along the row index (element (r,k) at src[k*ld + r]).  R = rows (MN extent) of the tile.  Each thread owns NV 16-byte
+// pieces of a [R x BK] block.  MN-major pieces are assigned so that a warp covers 16 rows x 8 k: 64-byte global segments,
+// and the transposing scalar stores spread over 16 banks.
 template <bool KC, int R>
-struct Operand {
-  static constexpr int VEC = R * BK / 4;
-  static constexpr int NV = (VEC + NPRODUCER - 1) / NPRODUCER;
-  // rounded to 1 KiB so that every buffer (the swizzled MN-major ones need 512 B atoms) starts aligned
-  static constexpr int BYTES = ((KC ? kmajor_bytes(R) : mnmajor_bytes(R)) + 1023) / 1024 * 1024;
+struct Loader {
+  static constexpr int NV = R * BK / 4 / NTHREADS;
+  static_assert(NV >= 1 && R % 16 == 0, "tile rows");
+  const float* base;
+  int64_t ld, step;  // step: pointer advance per block, in floats
+  int r0, rows;
+  float4 v[NV];
 
-  const float* gptr[NV];  // piece i of block 0
-  int soff[NV];           // byte offset inside an operand buffer; -1: this thread has no i-th piece
-  int kloc[NV];           // reduction index of the piece inside a block (K-major: first of 4; MN-major: the k row)
-  bool rok[NV];           // row index in range
-  int64_t step;           // pointer advance per block, in floats
-
-  __device__ __forceinline__ static int smem_off(int f) {
+  __device__ __forceinline__ static void piece(int f, int& rr, int& kk) {
     if (KC) {
-      const int r = f / (BK / 4), kc = f % (BK / 4);
-      return kc * kmajor_lbo(R) + (r >> 3) * 128 + (r & 7) * 16;
+      rr = f >> 3;
+      kk = (f & 7) * 4;
+    } else {
+      const int lane = f & 31, w = f >> 5, G = R / 16;
+      rr = ((w % G) * 4 + (lane & 3)) * 4;
+      kk = (w / G) * 8 + (lane >> 2);
     }
-    const int k = f / (R / 4), rc = f % (R / 4);  // rc: group of 4 consecutive row indices
-    return (rc >> 3) * MN_LBO + (k >> 2) * MN_SBO + (k & 3) * 128 + ((((rc >> 1) & 3) ^ (k & 3)) << 5) + (rc & 1) * 16;
   }
-  __device__ __forceinline__ void init(const float* __restrict__ src, int64_t ld, int r0, int rows, int k0) {
-    step = KC ? (int64_t)BK : (int64_t)BK * ld;
+  __device__ __forceinline__ void init(const float* __restrict__ src, int64_t ld_, int r0_, int rows_, int k0) {
+    ld = ld_;
+    r0 = r0_;
+    rows = rows_;
+    step = KC ? (int64_t)BK : (int64_t)BK * ld_;
+    base = KC ? src + k0 : src + (int64_t)k0 * ld_;
+  }
+  // krem = reduction elements left from this block's start
+  __device__ __forceinline__ void load(int kb, int krem) {
+    const float* blk = base + kb * step;
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
-      const int f = threadIdx.x + i * NPRODUCER;
-      soff[i] = -1;
-      gptr[i] = src;
-      kloc[i] = 0;
-      rok[i] = false;
-      if (f < VEC) {
-        soff[i] = smem_off(f);
-        if (KC) {
-          const int r = f / (BK / 4), kc = f % (BK / 4);
-          kloc[i] = kc * 4;
-          rok[i] = (r0 + r) < rows;
-          gptr[i] = src + (int64_t)(rok[i] ? r0 + r : 0) * ld + k0 + kc * 4;
-        } else {
-          const int k = f / (R / 4), rc = f % (R / 4);
-          kloc[i] = k;
-          rok[i] = (r0 + rc * 4) < rows;                       // rows % 4 == 0
-          gptr[i] = src + (int64_t)(k0 + k) * ld + (rok[i] ? r0 + rc * 4 : 0);
+      int rr, kk;
+      piece(threadIdx.x + i * NTHREADS, rr, kk);
+      const int gr = r0 + rr;
+      float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (KC) {
+        if (gr < rows) {
+          const float* p = blk + (int64_t)gr * ld + kk;
+          if (kk + 3 < krem) x = __ldg(reinterpret_cast<const float4*>(p));
+          else if (kk < krem) {
+            x.x = __ldg(p);
+            if (kk + 1 < krem) x.y = __ldg(p + 1);
+            if (kk + 2 < krem) x.z = __ldg(p + 2);
+          }
+        }
+      } else if (kk < krem && gr < rows) {
+        const float* p = blk + (int64_t)kk * ld + gr;
+        if (gr + 3 < rows) x = __ldg(reinterpret_cast<const float4*>(p));
+        else {
+          x.x = __ldg(p);
+          if (gr + 1 < rows) x.y = __ldg(p + 1);
+          if (gr + 2 < rows) x.z = __ldg(p + 2);
+        }
+      }
+      v[i] = x;
+    }
+  }
+  __device__ __forceinline__ void store(uint8_t* hi, uint8_t* lo) const {
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+      int rr, kk;
+      piece(threadIdx.x + i * NTHREADS, rr, kk);
+      const float4 x = v[i];
+      const float4 h = make_float4(tf32_trunc(x.x), tf32_trunc(x.y), tf32_trunc(x.z), tf32_trunc(x.w));
+      const float4 l = make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
+      if (KC) {
+        const int o = sw128_off(rr, kk);
+        *reinterpret_cast<float4*>(hi + o) = h;
+        *reinterpret_cast<float4*>(lo + o) = l;
+      } else {
+        const float hv[4] = {h.x, h.y, h.z, h.w}, lv[4] = {l.x, l.y, l.z, l.w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int o = sw128_off(rr + q, kk);
+          *reinterpret_cast<float*>(hi + o) = hv[q];
+          *reinterpret_cast<float*>(lo + o) = lv[q];
         }
       }
     }
   }
-  // krem = reduction elements left from this block's start (kend - k0 - kb*BK); kend % 4 == 0 for K-major sources
-  __device__ __forceinline__ void issue(int kb, int krem, uint8_t* raw) const {
-    const uint32_t base = smem_u32(raw);
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      if (soff[i] >= 0) {
-        const bool ok = rok[i] && kloc[i] < krem;
-        cp_async16(base + soff[i], ok ? gptr[i] + kb * step : gptr[i], ok ? 16u : 0u);  // 0 bytes: nothing is read, the 16 B are zero-filled
-      }
-    }
-  }
-  __device__ __forceinline__ void make_lo(const uint8_t* raw, uint8_t* lo) const {
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      if (soff[i] >= 0) {
-        const float4 v = *reinterpret_cast<const float4*>(raw + soff[i]);
-        float4 l;
-        l.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-        l.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-        l.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-        l.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-        *reinterpret_cast<float4*>(lo + soff[i]) = l;
-      }
-    }
-  }
-  // descriptor of k-step j (8 reduction elements) inside a staged buffer
-  __device__ __forceinline__ static uint64_t desc(uint32_t base, int j) {
-    if (KC) return umma_desc(base + 2 * j * kmajor_lbo(R), kmajor_lbo(R), 128);
-    return umma_desc(base + j * 2 * MN_SBO, MN_LBO, MN_SBO, 1);  // k-step = 8 k = two 4-deep atoms
-  }
 };
 
-template <bool A_KC, bool B_KC, int BN>
-__host__ __device__ constexpr int smem_bytes() { return (NRAW + NLO) * (Operand<A_KC, BM>::BYTES + Operand<B_KC, BN>::BYTES) + 1024; }
+template <int BN>
+struct TileCfg {
+  static constexpr int A_BYTES = BM * BK * 4;  // 16 KiB per buffer
+  static constexpr int B_BYTES = BN * BK * 4;
+  static constexpr int STAGE = 2 * (A_BYTES + B_BYTES);  // [A hi | A lo | B hi | B lo]
+  static constexpr int SLD = BN + 4;                     // epilogue staging row stride (16-byte aligned rows)
+  static constexpr int EPI = BM * SLD * 4 + BM * 16 * 4;  // staging tile + the hooks' [128][Q <= 16] slice
+  static constexpr int RING = 2 * STAGE;
+  static constexpr int SMEM = (RING > EPI ? RING : EPI) + 1024;  // + alignment slack of the 1024-byte swizzle atoms
+  // two CTAs per SM at BN = 64 (96 KiB of stages, <= 128 registers), one at BN = 128
+  static constexpr int MIN_BLOCKS = BN <= 64 ? 2 : 1;
+};
 
-// C[m, n] = sum_r A(m, r) * B(n, r) over r in [kbeg, kend) of this split.
-// Warp roles: warps 0..7 = producers (global -> registers -> hi/lo split -> smem stage, then the epilogue),
-// warp 8 = MMA issuer.  Stages are handed over with mbarriers only (full[s]: 8 producer-warp arrivals,
-// empty[s]: tcgen05.commit), so producers run up to NSTAGE blocks ahead of the tensor core and no block-wide
-// barrier sits in the main loop.
+// Epilogue: `stage` holds the raw tile [128][SLD] (sum of both accumulators).  The 256 threads write it out
+// row-contiguously, applying bias / ReLU / mask on the way, then run the fused column reductions.
+template <int BN>
+__device__ __forceinline__ void tile_epilogue(float* stage, const float* s_bias, bool s_bias_on, int m0, int n0, int M, int N,
+                                              float* __restrict__ C, int64_t ldc, const TcEpilogue& ep) {
+  constexpr int SLD = TileCfg<BN>::SLD;
+  constexpr int C4 = BN / 4;
+  constexpr int UNR = 4;  // independent row pieces per thread and trip: keeps the mask loads in flight together
+  const int rows_here = min(BM, M - m0);
+  const int total = rows_here * C4;
+  const bool vec_ok = ((ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(C) & 15) == 0);
+  const bool mvec_ok = ep.mask_src && ((ep.ldm & 3) == 0) && ((reinterpret_cast<uintptr_t>(ep.mask_src) & 15) == 0);
+  const bool want_hooks = ep.hooks.colsum || ep.hooks.stats || ep.hooks.S;
+  for (int base = threadIdx.x; base < total; base += NTHREADS * UNR) {
+    float4 o[UNR], mk[UNR];
+    int gm[UNR], gn[UNR];
+    bool live[UNR];
+#pragma unroll
+    for (int u = 0; u < UNR; ++u) {
+      const int idx = base + u * NTHREADS;
+      const int r = idx / C4, c4 = idx - r * C4;
+      gm[u] = m0 + r;
+      gn[u] = n0 + c4 * 4;
+      live[u] = idx < total && gn[u] < N;
+      mk[u] = make_float4(1.f, 1.f, 1.f, 1.f);
+      if (live[u]) {
+        o[u] = *reinterpret_cast<const float4*>(stage + r * SLD + c4 * 4);
+        if (ep.mask_src) {
+          const float* mp = ep.mask_src + (int64_t)gm[u] * ep.ldm + gn[u];
+          if (mvec_ok && gn[u] + 3 < N) mk[u] = *reinterpret_cast<const float4*>(mp);
+          else {
+            mk[u].x = mp[0];
+            mk[u].y = gn[u] + 1 < N ? mp[1] : 1.f;
+            mk[u].z = gn[u] + 2 < N ? mp[2] : 1.f;
+            mk[u].w = gn[u] + 3 < N ? mp[3] : 1.f;
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < UNR; ++u) {
+      if (!live[u]) continue;
+      float ov[4] = {o[u].x, o[u].y, o[u].z, o[u].w};
+      const float mv[4] = {mk[u].x, mk[u].y, mk[u].z, mk[u].w};
+      const float4 b4 = s_bias_on ? *reinterpret_cast<const float4*>(s_bias + (gn[u] - n0)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      const float bv[4] = {b4.x, b4.y, b4.z, b4.w};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        if (s_bias_on) ov[q] += bv[q];
+        if (ep.relu) ov[q] = fmaxf(ov[q], 0.f);
+        ov[q] = mv[q] > 0.f ? ov[q] : 0.f;
+      }
+      if (want_hooks)  // keep the final values in the staging tile for the column reductions below
+        *reinterpret_cast<float4*>(stage + (gm[u] - m0) * SLD + (gn[u] - n0)) = make_float4(ov[0], ov[1], ov[2], ov[3]);
+      float* dst = C + (int64_t)gm[u] * ldc + gn[u];
+      if (gn[u] + 3 < N && vec_ok) {
+        if (ep.atomic) atomicAdd(reinterpret_cast<float4*>(dst), make_float4(ov[0], ov[1], ov[2], ov[3]));
+        else *reinterpret_cast<float4*>(dst) = make_float4(ov[0], ov[1], ov[2], ov[3]);
+      } else {
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          if (gn[u] + q < N) {
+            if (ep.atomic) atomicAdd(dst + q, ov[q]); else dst[q] = ov[q];
+          }
+      }
+    }
+  }
+  // fused column reductions over the final tile: thread c owns output column n0 + c (conflict-free smem column walks),
+  // one atomic per (CTA, column[, q])
+  if (want_hooks) {
+    float* sS = stage + BM * SLD;  // [128][Q] slice of the per-row weights, behind the staging tile
+    if (ep.hooks.S)
+      for (int i = threadIdx.x; i < rows_here * ep.hooks.Q; i += NTHREADS) sS[i] = ep.hooks.S[(int64_t)m0 * ep.hooks.Q + i];
+    __syncthreads();
+    const int c = threadIdx.x;
+    if (c < BN && n0 + c < N) {
+      const int Q = ep.hooks.Q;
+      float s1 = 0.f;
+      double d1 = 0.0, d2 = 0.0;
+      float tq[16];
+#pragma unroll
+      for (int q = 0; q < 16; ++q) tq[q] = 0.f;
+      for (int r = 0; r < rows_here; ++r) {
+        const float v = stage[r * SLD + c];
+        s1 += v;
+        if (ep.hooks.stats) { d1 += (double)v; d2 += (double)v * (double)v; }
+        if (ep.hooks.S) {
+#pragma unroll
+          for (int q = 0; q < 16; ++q)
+            if (q < Q) tq[q] = fmaf(sS[r * Q + q], v, tq[q]);
+        }
+      }
+      if (ep.hooks.colsum) atomicAdd(&ep.hooks.colsum[n0 + c], s1);
+      if (ep.hooks.stats) {
+        atomicAdd(&ep.hooks.stats[n0 + c], d1);
+        atomicAdd(&ep.hooks.stats[(int64_t)N + n0 + c], d2);
+      }
+      if (ep.hooks.S) {
+#pragma unroll
+        for (int q = 0; q < 16; ++q)
+          if (q < Q)
+            atomicAdd(q < ep.hooks.q_split ? &ep.hooks.gT[(int64_t)q * ep.hooks.ldt + n0 + c]
+                                           : &ep.hooks.gT2[(int64_t)(q - ep.hooks.q_split) * ep.hooks.ldt + n0 + c], tq[q]);
+      }
+    }
+  }
+}
+
+// C[m, n] = sum_r A(m, r) * B(n, r) over r in [kbeg, kend) of this split (split z stores at C + z * ep.split_stride).
 template <bool A_KC, bool B_KC, int BN>
-__global__ void __launch_bounds__(NTHREADS, 1)
+__global__ void __launch_bounds__(NTHREADS, TileCfg<BN>::MIN_BLOCKS)
 k_gemm_3xtf32(const float* __restrict__ A, int64_t lda, const float* __restrict__ B, int64_t ldb, float* __restrict__ C, int64_t ldc,
               int M, int N, int K, int k_per_split, TcEpilogue ep) {
-  using OpA = Operand<A_KC, BM>;
-  using OpB = Operand<B_KC, BN>;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(8) uint64_t full_bar[NLO], raw_empty[NRAW], lo_empty[NLO], acc_bar;
-  __shared__ uint32_t tmem_base_s;
-  __shared__ __align__(16) float s_bias[BN];  // this tile's bias slice (zero past N), loaded once at the prologue
+  static_assert(BN % 64 == 0 && BN <= 128, "column halves of 64 (wgmma N); two accumulators of BN / 2 registers each");
+  using Cfg = TileCfg<BN>;
+  constexpr int NH = BN / 64;
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(16) float s_bias[BN];
+  // the swizzle pattern is a function of the address bits: stages start on 1024-byte boundaries
+  uint8_t* smem = smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023);
+  auto a_hi = [&](int s) { return smem + s * Cfg::STAGE; };
+  auto a_lo = [&](int s) { return a_hi(s) + Cfg::A_BYTES; };
+  auto b_hi = [&](int s) { return a_hi(s) + 2 * Cfg::A_BYTES; };
+  auto b_lo = [&](int s) { return b_hi(s) + Cfg::B_BYTES; };
 
-  uint8_t* bufs = smem;
-  constexpr int STAGE_BYTES = OpA::BYTES + OpB::BYTES;
-  auto a_hi = [&](int kb) { return bufs + (kb % NRAW) * STAGE_BYTES; };              // raw fp32 = hi operand
-  auto b_hi = [&](int kb) { return a_hi(kb) + OpA::BYTES; };
-  auto a_lo = [&](int kb) { return bufs + (NRAW + kb % NLO) * STAGE_BYTES; };
-  auto b_lo = [&](int kb) { return a_lo(kb) + OpA::BYTES; };
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
   const int kbeg = blockIdx.z * k_per_split;
   const int kend = min(K, kbeg + k_per_split);
   const int nkb = (kend - kbeg + BK - 1) / BK;
-  if (warp == 0) TC_TRACE(0);
   const bool s_bias_on = ep.bias != nullptr && blockIdx.z == 0;
 
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)),
-                 "r"((uint32_t)tmem_cols<BN>())
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (threadIdx.x == 32) {
-    for (int s = 0; s < NLO; ++s) {
-      mbar_init(smem_u32(&full_bar[s]), NPRODUCER / 32);
-      mbar_init(smem_u32(&lo_empty[s]), 1);
-    }
-    for (int s = 0; s < NRAW; ++s) mbar_init(smem_u32(&raw_empty[s]), 1);
-    mbar_init(smem_u32(&acc_bar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = tmem_base_s;
-  constexpr uint32_t idesc = umma_idesc(BM, BN, !A_KC, !B_KC);
-  // everything above (TMEM allocation, barrier init) is independent of the previous kernel's output
   pdl_prologue();
-  if (threadIdx.x < NPRODUCER)
-    for (int i = threadIdx.x; i < BN; i += NPRODUCER) s_bias[i] = (s_bias_on && n0 + i < N) ? ep.bias[n0 + i] : 0.f;
-  if (warp == 0) TC_TRACE(1);
+  for (int i = threadIdx.x; i < BN; i += NTHREADS) s_bias[i] = (s_bias_on && n0 + i < N) ? ep.bias[n0 + i] : 0.f;
 
-  if (warp < NPRODUCER / 32) {
-    // ---------------- producers ----------------
-    // block kb: wait for its raw stage, cp.async the raw pieces (they double as the hi operand); then finish block
-    // kb-AHEAD: its cp.async group has landed, derive lo from this thread's own pieces and publish it.
-    OpA pa;
-    OpB pb;
-    pa.init(A, lda, m0, M, kbeg);
-    pb.init(B, ldb, n0, N, kbeg);
-    auto publish = [&](int j) {
-      if (j >= NLO) mbar_wait(smem_u32(&lo_empty[j % NLO]), ((j / NLO) - 1) & 1);  // MMAs of block j-NLO have read the lo stage
-      pa.make_lo(a_hi(j), a_lo(j));
-      pb.make_lo(b_hi(j), b_lo(j));
-      // No proxy fence here: on the producer side it drains the thread's whole memory pipeline, i.e. the cp.async
-      // groups still in flight, and turns the main loop into one L2 round trip per block (measured).  The
-      // mbarrier arrive (release) / wait (acquire) pair orders these generic-proxy writes before the MMA
-      // warp's fence.proxy.async, which then orders them before its tcgen05.mma reads.
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&full_bar[j % NLO]));
-    };
-#pragma unroll 1
-    for (int kb = 0; kb < nkb; ++kb) {
-      if (kb >= NRAW) mbar_wait(smem_u32(&raw_empty[kb % NRAW]), ((kb / NRAW) - 1) & 1);  // MMAs of block kb-NRAW are done
-      pa.issue(kb, kend - kbeg - kb * BK, a_hi(kb));
-      pb.issue(kb, kend - kbeg - kb * BK, b_hi(kb));
-      cp_async_commit();
-      if (kb >= AHEAD) {
-        cp_async_wait<AHEAD>();  // all but the newest AHEAD groups are complete -> block kb-AHEAD has landed
-        publish(kb - AHEAD);
-        if (warp == 0 && kb == AHEAD) TC_TRACE(2);  // first block published
-      }
-    }
-    cp_async_wait<0>();
-    for (int j = (nkb > AHEAD ? nkb - AHEAD : 0); j < nkb; ++j) publish(j);
-    if (warp == 0) TC_TRACE(3);  // last block published
-  } else {
-    // ---------------- MMA issuer ----------------
-#pragma unroll 1
-    for (int kb = 0; kb < nkb; ++kb) {
-      mbar_wait(smem_u32(&full_bar[kb % NLO]), (kb / NLO) & 1);
-      fence_async_smem();  // generic-proxy writes observed through the barrier -> async proxy (tensor core reads)
-      tc_fence_after();
-      if (kb == 0) TC_TRACE(4);        // MMA warp: first stage ready
-      if (kb == nkb - 1) TC_TRACE(5);  // MMA warp: last stage ready
-      if (lane == 0) {
-        const uint32_t ah = smem_u32(a_hi(kb)), al = smem_u32(a_lo(kb)), bh = smem_u32(b_hi(kb)), bl = smem_u32(b_lo(kb));
+  Loader<A_KC, BM> la;
+  Loader<B_KC, BN> lb;
+  la.init(A, lda, m0, M, kbeg);
+  lb.init(B, ldb, n0, N, kbeg);
+
+  float acc[NH][32], accx[NH][32];  // hi*hi chain | cross terms
 #pragma unroll
-        for (int j = 0; j < BK / 8; ++j) {
-          const uint32_t first = (kb == 0 && j == 0) ? 0u : 1u;
-          umma_tf32(tmem_acc + BN, OpA::desc(al, j), OpB::desc(bh, j), idesc, first);  // cross terms -> second accumulator
-          umma_tf32(tmem_acc + BN, OpA::desc(ah, j), OpB::desc(bl, j), idesc, 1u);
-          umma_tf32(tmem_acc, OpA::desc(ah, j), OpB::desc(bh, j), idesc, first);
-        }
-        umma_commit(smem_u32(&lo_empty[kb % NLO]));     // both rings are released by the completion of these MMAs
-        umma_commit(smem_u32(&raw_empty[kb % NRAW]));
-        if (kb == nkb - 1) umma_commit(smem_u32(&acc_bar));  // accumulators complete
+  for (int h = 0; h < NH; ++h)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[h][i] = accx[h][i] = 0.f;
+
+  if (nkb > 0) {
+    la.load(0, kend - kbeg);
+    lb.load(0, kend - kbeg);
+    la.store(a_hi(0), a_lo(0));
+    lb.store(b_hi(0), b_lo(0));
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor cores
+  }
+#pragma unroll 1
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int s = kb & 1;
+    __syncthreads();  // stage s is complete; every wgmma of block kb - 1 (stage s ^ 1) has retired
+    const bool more = kb + 1 < nkb;
+    if (more) {  // next block's global loads fly under this block's MMAs
+      la.load(kb + 1, kend - kbeg - (kb + 1) * BK);
+      lb.load(kb + 1, kend - kbeg - (kb + 1) * BK);
+    }
+    const uint32_t ah = smem_u32(a_hi(s)) + wg * (64 * 128), al = smem_u32(a_lo(s)) + wg * (64 * 128);
+    const uint32_t bh = smem_u32(b_hi(s)), bl = smem_u32(b_lo(s));
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < BK / 8; ++j) {  // k-step j: 8 fp32 = 32 bytes into the 128-byte swizzle row
+#pragma unroll
+      for (int h = 0; h < NH; ++h) {
+        const uint32_t bo = h * (64 * 128) + j * 32;
+        wgmma_tf32_m64n64k8(accx[h], gmma_desc_sw128(al + j * 32), gmma_desc_sw128(bh + bo));
+        wgmma_tf32_m64n64k8(accx[h], gmma_desc_sw128(ah + j * 32), gmma_desc_sw128(bl + bo));
+        wgmma_tf32_m64n64k8(acc[h], gmma_desc_sw128(ah + j * 32), gmma_desc_sw128(bh + bo));
       }
-      __syncwarp();
+    }
+    wgmma_commit();
+    if (more) {
+      la.store(a_hi(s ^ 1), a_lo(s ^ 1));
+      lb.store(b_hi(s ^ 1), b_lo(s ^ 1));
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    }
+    wgmma_wait_all();
+#pragma unroll
+    for (int h = 0; h < NH; ++h) {
+      fence_acc(acc[h]);
+      fence_acc(accx[h]);
     }
   }
-  if (warp >= NPRODUCER / 32) {
-    // the MMA warp only has to stay alive until TMEM is released
-    tc_fence_before();
-    __syncthreads();
-    return;
-  }
-  if (nkb > 0) mbar_wait(smem_u32(&acc_bar), 0);
-  tc_fence_after();
-  if (warp == 0) TC_TRACE(6);  // accumulators complete, epilogue starts
+  __syncthreads();  // the stages are free: the staging tile reuses them
 
-  tc_epilogue<BN>(smem, s_bias, s_bias_on, tmem_acc, nkb, m0, n0, M, N, C, ldc, ep);
-  if (warp == 0) TC_TRACE(7);  // warp 0 epilogue done
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) TC_TRACE(8);  // all epilogue warps done
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "r"((uint32_t)tmem_cols<BN>()) : "memory");
+  // accumulator fragment of wgmma m64nN (f32): register 4i + j of lane l in warp w of the warpgroup holds
+  // row 16 w + l / 4 + 8 (j / 2), column 8 i + 2 (l % 4) + (j % 2)
+  float* stage = reinterpret_cast<float*>(smem);
+  {
+    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int col = h * 64 + i * 8 + (lane & 3) * 2;
+        *reinterpret_cast<float2*>(stage + row * Cfg::SLD + col) =
+            make_float2(acc[h][4 * i] + accx[h][4 * i], acc[h][4 * i + 1] + accx[h][4 * i + 1]);
+        *reinterpret_cast<float2*>(stage + (row + 8) * Cfg::SLD + col) =
+            make_float2(acc[h][4 * i + 2] + accx[h][4 * i + 2], acc[h][4 * i + 3] + accx[h][4 * i + 3]);
+      }
   }
+  __syncthreads();
+  tile_epilogue<BN>(stage, s_bias, s_bias_on, m0, n0, M, N, C + (int64_t)blockIdx.z * ep.split_stride, ldc, ep);
 }
 
 // gb[n] = sum_m gy[m][n]: 32 columns x 8 row-lanes per block, coalesced row sweeps, smem fold, one atomic per column
@@ -303,44 +403,12 @@ k_colsum_tc(const float* __restrict__ gy, int64_t ld, int M, int N, int rows_per
   }
 }
 
-// float4 variant (a lane owns four adjacent columns: 512-byte warp loads, a quarter of the load instructions per byte)
-__global__ void __launch_bounds__(256)
-k_colsum_tc_v4(const float* __restrict__ gy, int64_t ld, int M, int N4, int rows_per_block, float* __restrict__ gb) {
-  pdl_prologue();
-  __shared__ float4 red[8][32];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int n4 = blockIdx.x * 32 + lane;
-  const int r0 = blockIdx.y * rows_per_block, r1 = min(M, r0 + rows_per_block);
-  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (n4 < N4) {
-#pragma unroll 4
-    for (int r = r0 + w; r < r1; r += 8) {
-      const float4 v = *reinterpret_cast<const float4*>(gy + (int64_t)r * ld + 4 * n4);
-      a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
-    }
-  }
-  red[w][lane] = a;
-  __syncthreads();
-  if (w == 0 && n4 < N4) {
-    float4 t = red[0][lane];
-#pragma unroll
-    for (int k = 1; k < 8; ++k) {
-      const float4 v = red[k][lane];
-      t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
-    }
-    atomicAdd(&gb[4 * n4], t.x);
-    atomicAdd(&gb[4 * n4 + 1], t.y);
-    atomicAdd(&gb[4 * n4 + 2], t.z);
-    atomicAdd(&gb[4 * n4 + 3], t.w);
-  }
-}
-
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 template <bool A_KC, bool B_KC, int BN>
 int launch(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N, int K, int splits,
            int k_per_split, const TcEpilogue& ep, cudaStream_t st) {
-  constexpr int smem = smem_bytes<A_KC, B_KC, BN>();
+  constexpr int smem = TileCfg<BN>::SMEM;
   static bool configured = false;
   if (!configured) {
     PGNN_CUDA(cudaFuncSetAttribute(k_gemm_3xtf32<A_KC, B_KC, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -352,64 +420,23 @@ int launch(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, i
   return PGNN_OK;
 }
 
-// Tile width.  Measured (profiles/r01_gemm_phases.md): the main loop runs at the rate one SM can pull operands
-// (~26 GB/s per SM at DRAM latency, all producer designs alike), so per-CTA time ~ (128 + BN) bytes per block.
-//   * if some width covers the problem in ONE wave (<= 148 CTAs incl. splits), take the narrowest such width:
-//     least work per CTA, most SMs busy;
-//   * otherwise (many waves) operand re-reads dominate: take the widest width with <= 15% padding waste.
-// `kk`: both operands reduction-contiguous on the TMA kernel, whose B box is [BN rows x 32 k] for any BN % 16 == 0; there the
-// widths 112 and 208 exist as well: N = 300 tiles as 3 x 112 (11% padding instead of 28% with 3 x 128) and N = 600 as 3 x 208
-// (4% instead of 12% with 3 x 224) — the tensor time of a block is proportional to BN.  The MN-major boxes (32 rows each) and
-// the cp.async kernel need BN % 32 == 0.
-inline int pick_bn(int M, int N, int splits, bool kk = false) {
-  if (const char* e = getenv("PGNN_BN")) {  // development override
-    const int v = atoi(e);
-    if (v == 64 || v == 128 || v == 160 || v == 224 || (kk && (v == 112 || v == 208))) return v;
-  }
-  const int cand_kk[6] = {64, 112, 128, 160, 208, 224}, cand_32[4] = {64, 128, 160, 224};
-  const int* cand = kk ? cand_kk : cand_32;
-  const int nc = kk ? 6 : 4;
+// Tile width: the one with the least per-SM work over the whole grid, waves x (BN x CTAs resident per SM); a BN = 64
+// CTA holds half the shared memory and registers of a BN = 128 one, so two of them share an SM.  Ties go to the wider
+// tile (fewer re-reads of the A rows).
+inline int pick_bn(int M, int N, int splits) {
   const int64_t mt = ceil_div(M, BM) * (splits > 0 ? splits : 1);
-  for (int i = 0; i < nc; ++i)
-    if (mt * ceil_div(N, cand[i]) <= kNumSMs) return cand[i];
-  for (int i = nc - 1; i >= 0; --i) {
-    const int bn = cand[i];
-    const int padded = (int)ceil_div(N, bn) * bn;
-    if (padded <= N + N * 15 / 100 || bn == 64) return bn;
-  }
-  return 64;
+  auto cost = [&](int bn, int per_sm) { return ceil_div(mt * ceil_div(N, bn), (int64_t)kNumSMs * per_sm) * bn * per_sm; };
+  return cost(64, TileCfg<64>::MIN_BLOCKS) < cost(128, TileCfg<128>::MIN_BLOCKS) ? 64 : 128;
 }
 
 template <bool A_KC, bool B_KC>
 int dispatch(int bn, const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N, int K, int splits,
              int k_per_split, const TcEpilogue& ep, cudaStream_t st) {
-  switch (bn) {
-    case 64: return launch<A_KC, B_KC, 64>(A, lda, B, ldb, C, ldc, M, N, K, splits, k_per_split, ep, st);
-    case 128: return launch<A_KC, B_KC, 128>(A, lda, B, ldb, C, ldc, M, N, K, splits, k_per_split, ep, st);
-    case 160: return launch<A_KC, B_KC, 160>(A, lda, B, ldb, C, ldc, M, N, K, splits, k_per_split, ep, st);
-    default: return launch<A_KC, B_KC, 224>(A, lda, B, ldb, C, ldc, M, N, K, splits, k_per_split, ep, st);
-  }
+  if (bn == 64) return launch<A_KC, B_KC, 64>(A, lda, B, ldb, C, ldc, M, N, K, splits, k_per_split, ep, st);
+  return launch<A_KC, B_KC, 128>(A, lda, B, ldb, C, ldc, M, N, K, splits, k_per_split, ep, st);
 }
 
 }  // namespace
-
-int pgnn_tma_gemm_kk(int bn, const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N, int K,
-                     const TcEpilogue& ep, cudaStream_t st);
-int pgnn_tma_gemm(bool a_mn, bool b_mn, int bn, const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M,
-                  int N, int K, int splits, int k_per_split, const TcEpilogue& ep, cudaStream_t st);
-
-static bool tma_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("PGNN_NO_TMA");
-    v = (e && e[0] == '1') ? 0 : 1;
-  }
-  return v == 1;
-}
-
-extern "C" __attribute__((visibility("default"))) int pgnn_debug_tc_trace(unsigned long long* host16) {
-  return cudaMemcpyFromSymbol(host16, g_tc_trace, sizeof(unsigned long long) * 16) == cudaSuccess ? 0 : -2;
-}
 
 // development entry: C[M,N] = sum_r A(m,r) B(n,r) with explicit operand majors (1 = reduction-contiguous)
 extern "C" __attribute__((visibility("default"))) int pgnn_debug_tc_gemm(int a_kc, int b_kc, int bn, const float* A, int64_t lda,
@@ -417,6 +444,7 @@ extern "C" __attribute__((visibility("default"))) int pgnn_debug_tc_gemm(int a_k
                                                                         int N, int K, void* stream) {
   TcEpilogue ep{nullptr, 0, nullptr, 0, 0, PgnnGemmHooks{}};
   cudaStream_t st = as_stream(stream);
+  if (lda % 4 || ldb % 4 || !aligned16(A) || !aligned16(B)) return PGNN_EUNSUPPORTED;
   if (a_kc && b_kc) return dispatch<true, true>(bn, A, lda, B, ldb, C, ldc, M, N, K, 1, K, ep, st);
   if (a_kc && !b_kc) return dispatch<true, false>(bn, A, lda, B, ldb, C, ldc, M, N, K, 1, K, ep, st);
   if (!a_kc && b_kc) return dispatch<false, true>(bn, A, lda, B, ldb, C, ldc, M, N, K, 1, K, ep, st);
@@ -428,10 +456,6 @@ int pgnn_tc_linear_fwd(const float* x, int64_t ldx, const float* w, const float*
                        float* y, int64_t ldy, cudaStream_t st, const PgnnGemmHooks* hooks) {
   if (K % 4 || ldx % 4 || !aligned16(x) || !aligned16(w) || !aligned16(y) || M < 1) return PGNN_EUNSUPPORTED;
   TcEpilogue ep{bias, relu, nullptr, 0, 0, hooks ? *hooks : PgnnGemmHooks{}};
-  if (tma_enabled()) {  // both operands reduction-contiguous: TMA-staged kernel (dense_tma.cu)
-    const int rc = pgnn_tma_gemm_kk(pick_bn((int)M, (int)N, 1, true), x, ldx, w, K, y, ldy, (int)M, (int)N, (int)K, ep, st);
-    if (rc != PGNN_EUNSUPPORTED) return rc;
-  }
   return dispatch<true, true>(pick_bn((int)M, (int)N, 1), x, ldx, w, K, y, ldy, (int)M, (int)N, (int)K, 1, (int)K, ep, st);
 }
 
@@ -440,22 +464,17 @@ int pgnn_tc_linear_bwd_x(const float* gy, int64_t ldgy, const float* w, int64_t 
                          int64_t ldr, float* gx, int64_t ldgx, cudaStream_t st, const PgnnGemmHooks* hooks) {
   if (K % 4 || ldgy % 4 || !aligned16(gy) || !aligned16(w) || !aligned16(gx) || M < 1) return PGNN_EUNSUPPORTED;
   TcEpilogue ep{nullptr, 0, relu_src, ldr, 0, hooks ? *hooks : PgnnGemmHooks{}};
-  if (tma_enabled()) {  // A reduction-contiguous, B = w row-index-contiguous (MN-major boxes)
-    const int rc = pgnn_tma_gemm(false, true, pick_bn((int)M, (int)K, 1), gy, ldgy, w, K, gx, ldgx, (int)M, (int)K, (int)N, 1, (int)N, ep, st);
-    if (rc != PGNN_EUNSUPPORTED) return rc;
-  }
-  if (N % 4) return PGNN_EUNSUPPORTED;  // the cp.async kernel moves 16-byte pieces along the reduction; TMA zero-fills ragged extents
   // output columns are K; the reduction runs over N; B(n_out = k, r = n) = w[r*K + k] is row-index contiguous
   return dispatch<true, false>(pick_bn((int)M, (int)K, 1), gy, ldgy, w, K, gx, ldgx, (int)M, (int)K, (int)N, 1, (int)N, ep, st);
 }
 
 // dgrad with the TRANSPOSED weight at hand: gx[M,K] = gy[M,N] . wT[K,N]^T — both operands reduction-contiguous, so the
-// TMA-staged kernel applies (encoder.cu transposes the 2L weight matrices once per backward)
+// operand tiles are stored without a transpose (encoder.cu transposes the 2L weight matrices once per backward)
 int pgnn_tc_linear_bwd_x_wt(const float* gy, int64_t ldgy, const float* wT, int64_t M, int64_t N, int64_t K, const float* relu_src,
                             int64_t ldr, float* gx, int64_t ldgx, cudaStream_t st, const PgnnGemmHooks* hooks) {
-  if (!tma_enabled() || N % 4 || ldgy % 4 || !aligned16(gy) || !aligned16(wT) || !aligned16(gx) || M < 1) return PGNN_EUNSUPPORTED;
+  if (N % 4 || ldgy % 4 || !aligned16(gy) || !aligned16(wT) || !aligned16(gx) || M < 1) return PGNN_EUNSUPPORTED;
   TcEpilogue ep{nullptr, 0, relu_src, ldr, 0, hooks ? *hooks : PgnnGemmHooks{}};
-  return pgnn_tma_gemm_kk(pick_bn((int)M, (int)K, 1, true), gy, ldgy, wT, N, gx, ldgx, (int)M, (int)K, (int)N, ep, st);
+  return dispatch<true, true>(pick_bn((int)M, (int)K, 1), gy, ldgy, wT, N, gx, ldgx, (int)M, (int)K, (int)N, 1, (int)N, ep, st);
 }
 
 // out[c][r] = in[r][c] for a batch of row-major matrices (weights: a few hundred KB each)
@@ -497,7 +516,7 @@ int pgnn_internal_transpose_batch(int count, const float* const* in, float* cons
 
 namespace {
 // out[i] = sum_s part[s][i]: folds the split-K partial tiles (plain coalesced stores from the GEMM epilogue instead of
-// ~4 M vector atomics per wgrad on the same 0.7 MB of output)
+// vector atomics on the same 0.7 MB of output)
 __global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__ part, int splits, int64_t n4, float* __restrict__ out) {
   pdl_prologue();
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
@@ -518,136 +537,71 @@ __global__ void __launch_bounds__(256) k_splitk_reduce(const float* __restrict__
     reinterpret_cast<float4*>(out)[i] = a;
   }
 }
-}  // namespace
 
-namespace {
 // tile width, split count and rows per split of the weight-gradient GEMM gw[N,K] = gy[M,N]^T . x[M,K]
 struct WgradPlan { int bn, tiles, splits, per; };
 WgradPlan wgrad_plan(int64_t M, int64_t N, int64_t K) {
   WgradPlan p;
-  p.bn = 224;  // the reduction is long and both operands are re-read per tile: widest tile with <= 15% padding
-  for (int c : {224, 160, 128, 64}) {
-    p.bn = c;
-    if ((int)ceil_div(K, c) * c <= K + K * 15 / 100) break;
-  }
+  p.bn = 128;  // the reduction is long and both operands are re-read per tile: the wider tile unless it pads > 15%
+  if ((int)ceil_div(K, 128) * 128 > K + K * 15 / 100) p.bn = 64;
   p.tiles = (int)(ceil_div(N, BM) * ceil_div(K, p.bn));
-  int splits = kNumSMs / p.tiles;  // floor: 150 CTAs on 148 SMs would run as two waves
-  // the tensor core accumulates with truncation: keep each TMEM chain <= 1024 rows, fold the rest in fp32
+  int splits = kNumSMs * TileCfg<128>::MIN_BLOCKS / p.tiles;  // floor: one more CTA than the chip holds would be a second wave
+  if (p.bn == 64) splits = kNumSMs * TileCfg<64>::MIN_BLOCKS / p.tiles;
+  // keep each accumulation chain <= 1024 rows, fold the rest in fp32
   if (splits < (int)ceil_div(M, 1024)) splits = (int)ceil_div(M, 1024);
   const int max_splits = (int)ceil_div(M, 2 * BK);
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;
-  p.per = (int)align_up(ceil_div(M, splits), 32);  // multiple of the TMA kernel's 32-deep block (and of BK)
+  p.per = (int)align_up(ceil_div(M, splits), BK);
   p.splits = (int)ceil_div(M, p.per);
   return p;
 }
 }  // namespace
 
-// floats of split-K workspace pgnn_tc_linear_bwd_w_ws needs for this problem: one partial tile set per split + the arrival counters
+// floats of split-K workspace pgnn_tc_linear_bwd_w_ws needs for this problem: one partial tile set per split
 int64_t pgnn_tc_wgrad_workspace_floats(int64_t M, int64_t N, int64_t K) {
   if (M < 1) M = 1;
   const WgradPlan p = wgrad_plan(M, N, K);
-  return (int64_t)p.splits * N * K + align_up(p.tiles, 4) + 64;
+  return (int64_t)p.splits * N * K;
 }
 
 // gw[N,K] = gy[M,N]^T . x[M,K]; gb[N] = column sums of gy.  `partials` (optional, >= splits*N*K floats): split-K partial
 // tiles are stored there and folded by one reduction kernel; without it the epilogue uses vector atomics.
 int pgnn_tc_linear_bwd_w_ws(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
-                            float* gb, float* partials, int64_t partial_floats, cudaStream_t st);
-
-int pgnn_tc_linear_bwd_w(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
-                         float* gb, cudaStream_t st) {
-  return pgnn_tc_linear_bwd_w_ws(gy, ldgy, x, ldx, M, N, K, gw, gb, nullptr, 0, st);
-}
-
-static int device_sm_count() {
-  static int n = -1;
-  if (n < 0) {
-    int dev = 0, v = 0;
-    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) n = v;
-    else n = 1;
-  }
-  return n;
-}
-static bool fold_in_kernel_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    // "separate" (default): the fold is its own launch (k_splitk_reduce) | "kernel": arrival-counter fold inside the GEMM.
-    // Measured on the masking step (B200, single stream): 1.206 ms with the separate fold, 1.227 ms with the in-kernel one —
-    // the CTAs that arrive early spin on their SM instead of exiting, which costs more than the launch it saves.
-    const char* e = getenv("PGNN_SPLITK_FOLD");
-    v = (e && e[0] == 'k') ? 1 : 0;
-  }
-  return v == 1;
-}
-
-int pgnn_tc_linear_bwd_w_ws2(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
-                             float* gb, float* partials, int64_t partial_floats, cudaStream_t st, bool in_kernel_fold_ok);
-
-int pgnn_tc_linear_bwd_w_ws(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
                             float* gb, float* partials, int64_t partial_floats, cudaStream_t st) {
-  return pgnn_tc_linear_bwd_w_ws2(gy, ldgy, x, ldx, M, N, K, gw, gb, partials, partial_floats, st, true);
-}
-
-// in_kernel_fold_ok = false: the partial tiles are folded by k_splitk_reduce.  Callers that run this GEMM CONCURRENTLY with other
-// full-chip kernels (the encoders' side stream) must pass false: CTAs of the in-kernel fold spin until all their siblings have
-// arrived, and a sibling queued behind another kernel's CTAs would keep the arrived ones idling on their SMs.
-int pgnn_tc_linear_bwd_w_ws2(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
-                             float* gb, float* partials, int64_t partial_floats, cudaStream_t st, bool in_kernel_fold_ok) {
   if (K % 4 || ldgy % 4 || ldx % 4 || !aligned16(gy) || !aligned16(x) || !aligned16(gw) || M < 1) return PGNN_EUNSUPPORTED;
-  if ((N % 4) && !tma_enabled()) return PGNN_EUNSUPPORTED;  // ragged N (e.g. 119 classes) only through the TMA boxes
   // output [N, K] (rows N = "M" of the MMA), reduction over the M node rows, split so the grid fills the chip
   const WgradPlan plan = wgrad_plan(M, N, K);
-  const int bn = plan.bn, tiles = plan.tiles, splits = plan.splits, per = plan.per;
-  int rc = PGNN_EUNSUPPORTED;
-  const bool two_phase = splits > 1 && partials && partial_floats >= (int64_t)splits * N * K && tma_enabled() && ((N * K) % 4 == 0);
-  if (two_phase) {
-    // split s writes its tile into partials[s] (the kernel offsets C by blockIdx.z * N * ldc through ep.split_stride)
+  const int bn = plan.bn, splits = plan.splits, per = plan.per;
+  int rc;
+  if (splits > 1 && partials && partial_floats >= (int64_t)splits * N * K && ((N * K) % 4 == 0)) {
+    // split s writes its tile into partials[s] (the kernel offsets C by blockIdx.z * ep.split_stride)
     TcEpilogue ep{nullptr, 0, nullptr, 0, 0, PgnnGemmHooks{}};
     ep.split_stride = N * K;
-    // The fold runs inside the GEMM when its whole grid is resident at once (one 220 KB CTA per SM): the counters sit behind
-    // the partial tiles in the workspace.
-    const int64_t ctr_floats = align_up(tiles, 4);
-    const bool in_kernel = in_kernel_fold_ok && fold_in_kernel_enabled() && (int64_t)tiles * splits <= device_sm_count() && (K % 4) == 0 &&
-                           partial_floats >= (int64_t)splits * N * K + ctr_floats;
-    if (in_kernel) {
-      unsigned int* ctr = reinterpret_cast<unsigned int*>(partials + (int64_t)splits * N * K);
-      PGNN_CUDA(cudaMemsetAsync(ctr, 0, sizeof(unsigned int) * tiles, st));
-      ep.fold_counter = ctr;
-      ep.fold_out = gw;
-    }
-    rc = pgnn_tma_gemm(true, true, bn, gy, ldgy, x, ldx, partials, K, (int)N, (int)K, (int)M, splits, per, ep, st);
-    if (rc == PGNN_OK && !in_kernel) {
-      const int64_t n4 = N * K / 4;
-      int blocks = (int)ceil_div(n4, 256);
-      if (blocks > kNumSMs * 4) blocks = kNumSMs * 4;
-      PGNN_CUDA(pgnn_launch(k_splitk_reduce, dim3(blocks), dim3(256), 0, st, partials, splits, n4, gw));
-      PGNN_LAUNCH_CHECK();
-    }
-  }
-  if (rc == PGNN_EUNSUPPORTED) {
+    rc = dispatch<false, false>(bn, gy, ldgy, x, ldx, partials, K, (int)N, (int)K, (int)M, splits, per, ep, st);
+    if (rc != PGNN_OK) return rc;
+    const int64_t n4 = N * K / 4;
+    int blocks = (int)ceil_div(n4, 256);
+    if (blocks > kNumSMs * 4) blocks = kNumSMs * 4;
+    PGNN_CUDA(pgnn_launch(k_splitk_reduce, dim3(blocks), dim3(256), 0, st, partials, splits, n4, gw));
+    PGNN_LAUNCH_CHECK();
+  } else {
     if (splits > 1) PGNN_CUDA(cudaMemsetAsync(gw, 0, sizeof(float) * N * K, st));
     TcEpilogue ep{nullptr, 0, nullptr, 0, splits > 1, PgnnGemmHooks{}};
-    if (tma_enabled()) rc = pgnn_tma_gemm(true, true, bn, gy, ldgy, x, ldx, gw, K, (int)N, (int)K, (int)M, splits, per, ep, st);
-    if (rc == PGNN_EUNSUPPORTED && (N % 4) == 0)
-      rc = dispatch<false, false>(bn, gy, ldgy, x, ldx, gw, K, (int)N, (int)K, (int)M, splits, per, ep, st);
-    if (rc == PGNN_EUNSUPPORTED) return rc;
+    rc = dispatch<false, false>(bn, gy, ldgy, x, ldx, gw, K, (int)N, (int)K, (int)M, splits, per, ep, st);
+    if (rc != PGNN_OK) return rc;
   }
-  if (rc != PGNN_OK) return rc;
   if (gb) {
     PGNN_CUDA(cudaMemsetAsync(gb, 0, sizeof(float) * N, st));
     const int rows_per = M >= 16384 ? 256 : 64;  // 8 rows per thread for small batches: the row loop is a latency chain
-    // the float4 variant measured slower at both sizes (N = 6 k: 51.6 vs 45.9 us per step; N = 32 k: 16.1 vs 14.1 us per launch): opt-in only
-    static const bool colsum_v4 = getenv("PGNN_COLSUM_V4") && getenv("PGNN_COLSUM_V4")[0] == '1';
-    if (colsum_v4 && N % 4 == 0 && ldgy % 4 == 0 && aligned16(gy)) {
-      dim3 g4((unsigned)ceil_div(N / 4, 32), (unsigned)ceil_div(M, rows_per));
-      PGNN_CUDA(pgnn_launch(k_colsum_tc_v4, dim3(g4), dim3(256), 0, st, gy, ldgy, (int)M, (int)(N / 4), rows_per, gb));
-      PGNN_LAUNCH_CHECK();
-      return PGNN_OK;
-    }
     dim3 g2((unsigned)ceil_div(N, 32), (unsigned)ceil_div(M, rows_per));
     PGNN_CUDA(pgnn_launch(k_colsum_tc, dim3(g2), dim3(256), 0, st, gy, ldgy, (int)M, (int)N, rows_per, gb));
     PGNN_LAUNCH_CHECK();
   }
   return PGNN_OK;
+}
+
+int pgnn_tc_linear_bwd_w(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
+                         float* gb, cudaStream_t st) {
+  return pgnn_tc_linear_bwd_w_ws(gy, ldgy, x, ldx, M, N, K, gw, gb, nullptr, 0, st);
 }

@@ -21,10 +21,6 @@ int pgnn_internal_aggregate_fwd(const float* x, int64_t ldx, const float* in_sca
                                 const float* S, int64_t Q, const float* T, const float* T2, int q_split, int64_t edge_off, float* out,
                                 int64_t ldo, cudaStream_t st, const PgnnBnFold* fold);
 
-int pgnn_tma_gin_gather_gemm(const float* x, int64_t ldx, const float* in_scale, const float* in_shift, const PgnnBnFold* fold, int in_relu,
-                             const int32_t* rowptr_t, const int32_t* nbr_t, const float* S, int Q, const float* T, const float* T2,
-                             int q_split, float* aggr, int64_t lda, const float* W, const float* bias, int relu, float* z1, int64_t ldz,
-                             int64_t M, int64_t N, int64_t K, unsigned int* tile_ctr, cudaStream_t st);
 int pgnn_internal_chem_onehot(const int64_t* x, int64_t n, int rows1, int rows2, float* onehot, int64_t ld, cudaStream_t st);
 
 int pgnn_tc_linear_fwd(const float*, int64_t, const float*, const float*, int64_t, int64_t, int64_t, int, float*, int64_t,
@@ -34,8 +30,6 @@ int pgnn_tc_linear_bwd_x(const float*, int64_t, const float*, int64_t, int64_t, 
 int pgnn_tc_linear_bwd_w(const float*, int64_t, const float*, int64_t, int64_t, int64_t, int64_t, float*, float*, cudaStream_t);
 int pgnn_tc_linear_bwd_w_ws(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
                             float* gb, float* partials, int64_t partial_floats, cudaStream_t st);
-int pgnn_tc_linear_bwd_w_ws2(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
-                             float* gb, float* partials, int64_t partial_floats, cudaStream_t st, bool in_kernel_fold_ok);
 int64_t pgnn_tc_wgrad_workspace_floats(int64_t M, int64_t N, int64_t K);
 int pgnn_tc_linear_bwd_x_wt(const float* gy, int64_t ldgy, const float* wT, int64_t M, int64_t N, int64_t K, const float* relu_src,
                             int64_t ldr, float* gx, int64_t ldgx, cudaStream_t st, const PgnnGemmHooks* hooks);
@@ -73,8 +67,6 @@ struct Ws {
   float *S, *h0, *scale, *shift, *mean, *invstd;  // scale/shift/mean/invstd: [L, D]
   float* onehot;                                   // [N, kOneHotLd]: atom-code one-hot rows (embedding gradient as a GEMM)
   double* bn_acc;                                  // [L][2][D] fp64 BatchNorm sums of the forward
-  unsigned int* tile_ctr;                          // [L][tiles] arrival counters of the fused gather + GEMM1 kernel (zeroed per forward)
-  int64_t tiles;
   float *aggr, *z1, *z2;                           // [L, N, D], [L, N, 2D], [L, N, D]
   float *gh, *gz2, *gz1, *gaggr;                   // backward temporaries
   float* wT;                                       // [L][2][2D*D]: mlp.0.weight^T, mlp.2.weight^T (dgrad B operands)
@@ -98,8 +90,6 @@ Ws carve(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
   w.h0 = c.take<float>(N * D);
   w.onehot = c.take<float>(N * kOneHotLd);
   w.bn_acc = c.take<double>(L * 2 * D);
-  w.tiles = ceil_div(N > 0 ? N : 1, 128);
-  w.tile_ctr = c.take<unsigned int>(L * w.tiles);
   w.scale = c.take<float>(L * D);
   w.shift = c.take<float>(L * D);
   w.mean = c.take<float>(L * D);
@@ -237,7 +227,6 @@ int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mea
   if (N == 0) return PGNN_OK;
   if (training && N < 1) return PGNN_EINVAL;
   Ws w = carve(workspace, N, E, L, D);
-  if (precision == 1) PGNN_CUDA(cudaMemsetAsync(w.tile_ctr, 0, sizeof(unsigned int) * L * w.tiles, as_stream(stream)));
   TRY(pgnn_graph_prep(edge_index, E, N, w.rowptr_t, w.nbr_t, w.eid_t, w.rowptr_s, w.nbr_s, w.eid_s, w.scratch, w.scratch_bytes, stream));
   TRY(pgnn_chem_edge_summary(edge_attr, w.rowptr_t, w.nbr_t, w.eid_t, N, PGNN_AGG_SUM, nullptr, w.S, stream));
   TRY(pgnn_chem_embed_fwd(x, (const float*)params[P_XEMB1], kAtomRows, (const float*)params[P_XEMB2], kChiralRows, N, D, w.h0, D, stream));
@@ -253,21 +242,11 @@ int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mea
     float* z1 = w.z1 + l * N * 2 * D;
     float* z2 = w.z2 + l * N * D;
     const bool last = (l == L - 1);
-    // gather + GEMM1.  Tensor path: ONE kernel (k_gin_gather_gemm): the column tiles of a row tile form a cluster that gathers the
-    // tile's rows together, then runs the GEMM on them (`aggr` is stored once: the backward's weight-gradient GEMM reads it).
-    int rc_f = PGNN_EUNSUPPORTED;
-    if (precision == 1)
-      rc_f = pgnn_tma_gin_gather_gemm(h, D, in_scale, in_shift, have_fold ? &fold : nullptr, in_scale != nullptr || have_fold, w.rowptr_t,
-                                      w.nbr_t, w.S, 9, (const float*)p[L_ET1], (const float*)p[L_ET2], 6, aggr, D,
-                                      (const float*)p[L_W1], (const float*)p[L_B1], 1, z1, 2 * D, N, 2 * D, D, w.tile_ctr + l * w.tiles, as_stream(stream));
-    if (rc_f == PGNN_EUNSUPPORTED) {
-      TRY(pgnn_internal_aggregate_fwd(h, D, in_scale, in_shift, in_scale != nullptr || have_fold, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_SUM,
-                                      nullptr, w.S, 9, (const float*)p[L_ET1], (const float*)p[L_ET2], 6, 0, aggr, D, as_stream(stream),
-                                      have_fold ? &fold : nullptr));
-      TRY(pgnn_linear_fwd(aggr, D, (const float*)p[L_W1], (const float*)p[L_B1], N, 2 * D, D, 1, z1, 2 * D, precision, stream));
-    } else if (rc_f != PGNN_OK) {
-      return rc_f;
-    }
+    // gather (the previous layer's BatchNorm + ReLU applied on load) + GEMM1
+    TRY(pgnn_internal_aggregate_fwd(h, D, in_scale, in_shift, in_scale != nullptr || have_fold, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_SUM,
+                                    nullptr, w.S, 9, (const float*)p[L_ET1], (const float*)p[L_ET2], 6, 0, aggr, D, as_stream(stream),
+                                    have_fold ? &fold : nullptr));
+    TRY(pgnn_linear_fwd(aggr, D, (const float*)p[L_W1], (const float*)p[L_B1], N, 2 * D, D, 1, z1, 2 * D, precision, stream));
     have_fold = false;
     // GEMM2; on the tensor path its epilogue also accumulates the BatchNorm batch statistics of z2 (fp64 atomics)
     bool stats_fused = false;
@@ -333,8 +312,8 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
   }
   PGNN_CHECK_ARG(g_node_rep && x);
   Ws w = carve(workspace, N, E, L, D);
-  // transposed copies of the 2L MLP weights: with them every dgrad has both operands reduction-contiguous and runs on
-  // the TMA-staged GEMM (dense_tma.cu) instead of the cp.async one
+  // transposed copies of the 2L MLP weights: with them every dgrad has both operands reduction-contiguous, and the GEMM
+  // stores its operand tiles without a transpose
   bool have_wT = false;
   if (precision == 1 && 2 * L <= 32) {
     const float* in[32];
@@ -376,7 +355,7 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
         PGNN_CUDA(cudaEventRecord(sc->gz2_ready[par], st));
         PGNN_CUDA(cudaStreamWaitEvent(wst, sc->gz2_ready[par], 0));
       }
-      int rc = pgnn_tc_linear_bwd_w_ws2(gz2, D, z1, 2 * D, N, D, 2 * D, grads + o[L_W2], nullptr, w.wpart, w.wpart_floats, wst, sc == nullptr);
+      int rc = pgnn_tc_linear_bwd_w_ws(gz2, D, z1, 2 * D, N, D, 2 * D, grads + o[L_W2], nullptr, w.wpart, w.wpart_floats, wst);
       if (rc == PGNN_OK) {
         if (sc) {
           PGNN_CUDA(cudaEventRecord(sc->w2_done[par], wst));
@@ -394,7 +373,7 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
           PGNN_CUDA(cudaEventRecord(sc->gz1_ready[par], st));
           PGNN_CUDA(cudaStreamWaitEvent(wst, sc->gz1_ready[par], 0));
         }
-        rc = pgnn_tc_linear_bwd_w_ws2(gz1, 2 * D, aggr, D, N, 2 * D, D, grads + o[L_W1], nullptr, w.wpart, w.wpart_floats, wst, sc == nullptr);
+        rc = pgnn_tc_linear_bwd_w_ws(gz1, 2 * D, aggr, D, N, 2 * D, D, grads + o[L_W1], nullptr, w.wpart, w.wpart_floats, wst);
         if (rc != PGNN_OK) return rc;
         if (sc) PGNN_CUDA(cudaEventRecord(sc->w1_done[par], wst));
         PGNN_CUDA(cudaMemsetAsync(grads + o[L_ET1], 0, sizeof(float) * 9 * D, st));  // the two tables are adjacent in the layout
@@ -433,7 +412,7 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
     PGNN_CUDA(cudaStreamWaitEvent(st, sc->join, 0));
   }
   // embedding tables: [120 + 3, D] = onehot^T . gh as a split-K weight-gradient GEMM (the two tables are adjacent in the flat
-  // layout); the vector-atomics kernel remains the fallback (FFMA precision, TMA unavailable)
+  // layout); the vector-atomics kernel remains the fallback (FFMA precision)
   int rc_e = PGNN_EUNSUPPORTED;
   if (precision == 1 && embed_gemm_enabled() && off[P_XEMB2] == off[P_XEMB1] + (int64_t)kAtomRows * D)
     rc_e = pgnn_tc_linear_bwd_w_ws(w.onehot, kOneHotLd, w.gh, D, N, kAtomRows + kChiralRows, D, grads + off[P_XEMB1], nullptr, w.wpart,

@@ -24,8 +24,6 @@ int pgnn_internal_aggregate_fwd(const float* x, int64_t ldx, const float* in_sca
 int pgnn_internal_chem_onehot(const int64_t* x, int64_t n, int rows1, int rows2, float* onehot, int64_t ld, cudaStream_t st);
 int pgnn_tc_linear_bwd_w_ws(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
                             float* gb, float* partials, int64_t partial_floats, cudaStream_t st);
-int pgnn_tc_linear_bwd_w_ws2(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
-                             float* gb, float* partials, int64_t partial_floats, cudaStream_t st, bool in_kernel_fold_ok);
 int64_t pgnn_tc_wgrad_workspace_floats(int64_t M, int64_t N, int64_t K);
 
 namespace {
@@ -317,8 +315,7 @@ int pgnn_chem_conv_backward(int conv_type, const void* const* params, const floa
     }
     int rc = PGNN_EUNSUPPORTED;
     if (precision == 1)
-      rc = pgnn_tc_linear_bwd_w_ws2(gxl, HD, hin, D, N, HD, D, grads + o[gat ? A_W : G_W], grads + o[gat ? A_B : G_B], w.wpart, w.wpart_floats, wst,
-                                    sc == nullptr);
+      rc = pgnn_tc_linear_bwd_w_ws(gxl, HD, hin, D, N, HD, D, grads + o[gat ? A_W : G_W], grads + o[gat ? A_B : G_B], w.wpart, w.wpart_floats, wst);
     if (rc == PGNN_EUNSUPPORTED) {
       if (sc) {
         PGNN_CUDA(cudaEventRecord(sc->join, wst));

@@ -457,7 +457,7 @@ int pgnn_gat_bwd(const float* g, int64_t ldg, const float* xl, int64_t num_nodes
   BwdWs w = carve(workspace, num_nodes, num_edges, H);
   PGNN_CUDA(cudaMemsetAsync(w.Bsum, 0, sizeof(float) * kQ * kMaxH, st));
   // PGNN_GAT_OCC=1: the 64-register build (four resident CTAs per SM instead of three; the kernel is a chain of dependent loads per
-  // warp, so resident warps are what it is short of) -- measured against the default in profiles/README.md
+  // warp, so resident warps are what it is short of); off by default
   static const bool occ4 = getenv("PGNN_GAT_OCC") && getenv("PGNN_GAT_OCC")[0] == '1';
 #define PGNN_GAT_BT(BIO_, MINB_)                                                                                                          \
   PGNN_CUDA(pgnn_launch(k_gat_bwd_target<BIO_, MINB_>, dim3(warp_grid(num_nodes)), dim3(256), 0, st, g, ldg, xl, num_nodes, (int)H, (int)D, att, T, \

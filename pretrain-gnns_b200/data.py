@@ -2,7 +2,7 @@
 host-collated batches (one pinned buffer, one asynchronous copy per batch) for callers that keep the reference's DataLoader.
 
 The reference collates on the host, one Python loop of `torch.cat`s per batch (chem/batch.py:17-52 BatchMasking,
-:141-210 BatchSubstructContext) inside DataLoader workers, then copies the batch to the GPU.  A B200 has 180 GB of
+:141-210 BatchSubstructContext) inside DataLoader workers, then copies the batch to the GPU.  An H100 has 80 GB of
 HBM: the whole pre-training set (ZINC15, 2M molecules x ~23 atoms: < 1 GB in the compact form below) stays resident and a
 batch is one `pgnn_collate_chem` call on a list of graph ids -- no host work, no H2D copy per step.
 """

@@ -21,7 +21,7 @@ _precision = _PRECISION.get(os.environ.get("PGNN_PRECISION", "tf32x3"), 1)
 
 
 def set_precision(name: str):
-    """'fp32' = FFMA SIMT GEMMs (exact fp32); 'tf32x3' = error-compensated 3xTF32 tcgen05 GEMMs."""
+    """'fp32' = FFMA SIMT GEMMs (exact fp32); 'tf32x3' = error-compensated 3xTF32 wgmma GEMMs."""
     global _precision
     _precision = _PRECISION[name]
 

@@ -1,4 +1,4 @@
-"""The `train()` bodies of the reference's pre-training scripts on the B200 modules — one callable per BASELINE config.
+"""The `train()` bodies of the reference's pre-training scripts on the library's modules — one callable per BASELINE config.
 
 Each class owns the modules the script builds, draws the synthetic batches of its config (SURVEY.md 8(d)) and, called
 on one device-resident batch, runs exactly what the script runs between `batch.to(device)` and `optimizer.step()`:

@@ -23,7 +23,7 @@ import torch
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), "..", ".."))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-from golden_util import PRETRAINED, input_checksum, pretrained_batch  # noqa: E402
+from golden_util import PRETRAINED, input_checksum, pretrained_batch, pretrained_rows  # noqa: E402
 from oracle import reference_runner  # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -45,7 +45,7 @@ def main():
         b = pretrained_batch(name)
         with torch.no_grad():
             y = model(b["x"], b["edge_index"], b["edge_attr"])
-        out[name + ":out_eval"] = y.numpy()
+        rows = pretrained_rows(y.shape[0])
         # the same forward in float64: the yardstick for how well conditioned the checkpoint is (the trained GIN's pre-BatchNorm
         # activations reach 1e5, and eval-mode BatchNorm turns a uniform absolute error of the Linear output into per-column errors)
         m64 = ref.GNN(5, 300, JK="last", drop_ratio=0, gnn_type=c["type"])
@@ -54,7 +54,12 @@ def main():
         with torch.no_grad():
             y64 = m64(b["x"].double() if b["x"].is_floating_point() else b["x"], b["edge_index"],
                       b["edge_attr"].double() if b["edge_attr"].is_floating_point() else b["edge_attr"])
-        out[name + ":d64"] = (y64 - y.double()).float().numpy()     # ref64 = out_eval + d64 (the difference is tiny: stored in fp32)
+        # a seeded sample of the rows is stored; the full tensor's scale goes with it so that errors keep their meaning
+        out[name + ":rows"] = rows.numpy()
+        out[name + ":n"] = np.int64(y.shape[0])
+        out[name + ":scale"] = np.float64(y64.abs().max())
+        out[name + ":out_eval"] = y[rows].numpy()
+        out[name + ":d64"] = (y64 - y.double())[rows].float().numpy()     # ref64 = out_eval + d64 (the difference is tiny: stored in fp32)
         out[name + ":input_checksum"] = input_checksum(b)
         out[name + ":sha256"] = np.frombuffer(hashlib.sha256(open(path, "rb").read()).digest(), dtype=np.uint8)
         print("%-14s N = %5d  max|out| = %8.3f  %s" % (name, y.shape[0], float(y.abs().max()), c["file"]))

@@ -40,13 +40,19 @@ def pretrained_batch(name):
     return syn.ppi_batch(c["graphs"], c["seed"], n_lo=80, n_hi=120, num_tasks=16)
 
 
+PRETRAINED_ROWS = 80   # output rows per checkpoint kept in tests/golden/pretrained.npz (a seeded sample: the file stays small)
+
+
+def pretrained_rows(n):
+    """The sampled output rows of a golden with n rows (make_golden_pretrained.py stores them, the tests read them back)."""
+    return torch.randperm(n, generator=torch.Generator().manual_seed(0))[:PRETRAINED_ROWS].sort().values
+
+
 def pretrained_state_dict(name):
-    """The checkpoint of PRETRAINED[name]: from /root/reference in the build container, from the staged copy on the GPU box."""
-    c = PRETRAINED[name]
-    for root in ("/root/reference", os.path.join(os.path.dirname(HERE), "oracle", "_ref", "weights")):
-        path = os.path.join(root, c["file"])
-        if os.path.isfile(path):
-            return torch.load(path, map_location="cpu", weights_only=True), path
+    """The checkpoint of PRETRAINED[name] from the copy __graft_entry__.build() stages under oracle/_ref/weights."""
+    path = os.path.join(os.path.dirname(HERE), "oracle", "_ref", "weights", PRETRAINED[name]["file"])
+    if os.path.isfile(path):
+        return torch.load(path, map_location="cpu", weights_only=True), path
     return None, None
 
 
@@ -170,7 +176,7 @@ def grad_close(mine, ref32, ref64, floor=1.0, gtol=2e-4, slack=4.0):
 # Full-size oracle parity (tests/test_gpu_parity_full.py): per-tensor bounds stated against what is measured.
 #
 # Forward outputs: the north_star bound |mine - ref32| <= 1e-4 + 1e-4 |ref32|, AND max|mine - ref64| <= OUT_REL x the
-# tensor's largest magnitude (measured on B200: 1-4e-6 for the 3xTF32 path; OUT_REL is ~10x that).
+# tensor's largest magnitude (OUT_REL is ~10x the 1-4e-6 the 3xTF32 path measures).
 # Gradients, per tensor: err = max|mine - ref64| / scale with scale = the tensor's own largest |ref64| (floored at 1e-3 of the
 # model's largest gradient; a structurally zero gradient -- a bias in front of train-mode BatchNorm -- is compared on the
 # model's scale).  Train-mode BatchNorm makes fp32 gradients ill-conditioned: the oracle's OWN fp32 run misses its fp64 run

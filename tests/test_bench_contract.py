@@ -1,4 +1,4 @@
-"""CPU: the bench's reference arm prints the contract's JSON line; the B200 arm refuses to run without a GPU."""
+"""CPU: the bench's reference arm prints the contract's JSON line; the GPU arm refuses to run without a GPU."""
 import json
 import os
 import subprocess
@@ -49,3 +49,29 @@ def test_b200_arm_needs_a_gpu():
         return
     r = _run("--steps", "1", "--warmup", "1")
     assert r.returncode != 0 and "no CPU fallback" in (r.stderr + r.stdout)
+
+
+def test_dump_outputs_files_dtypes_and_budget(tmp_path, monkeypatch):
+    """bench.dump_outputs: loss as float64, one float32 file per gradient; over the byte budget every array becomes a seeded sample
+    whose values and int64 indices together stay within it, and the same call gives the same sample."""
+    import numpy as np
+    import bench
+    g = torch.Generator().manual_seed(0)
+    loss = torch.tensor(1.25, dtype=torch.float64)
+    grads = [("a.weight", torch.randn(300, 200, generator=g)), ("a.bias", torch.randn(300, generator=g)), ("b.weight", None)]
+    bench.dump_outputs(str(tmp_path / "full"), loss, grads)
+    full = tmp_path / "full"
+    assert sorted(p.name for p in full.iterdir()) == ["grad.a.bias.npy", "grad.a.weight.npy", "loss.npy"]
+    assert np.load(full / "loss.npy").dtype == np.float64 and float(np.load(full / "loss.npy")[0]) == 1.25
+    w = np.load(full / "grad.a.weight.npy")
+    assert w.dtype == np.float32 and np.array_equal(w, grads[0][1].numpy())
+    monkeypatch.setattr(bench, "DUMP_BYTES", 64 << 10)   # far below the 241 KB of these arrays
+    for run in ("s1", "s2"):
+        bench.dump_outputs(str(tmp_path / run), loss, grads)
+        assert sum(p.stat().st_size for p in (tmp_path / run).iterdir()) <= bench.DUMP_BYTES
+    idx = np.load(tmp_path / "s1" / "grad.a.weight.idx.npy")
+    vals = np.load(tmp_path / "s1" / "grad.a.weight.npy")
+    assert idx.dtype == np.int64 and vals.dtype == np.float32 and idx.size == vals.size > 0
+    assert np.array_equal(vals, grads[0][1].numpy().reshape(-1)[idx])
+    for f in (tmp_path / "s1").iterdir():
+        assert np.array_equal(np.load(f), np.load(tmp_path / "s2" / f.name))

@@ -48,24 +48,22 @@ def test_state_dict_contract(domain, t):
         ("bio", "gin"): 2726100, ("bio", "gcn"): 467100, ("bio", "graphsage"): 467100, ("bio", "gat"): 941100}[(domain, t)]
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/chem/model_gin/masking.pth"), reason="reference tree absent")
 def test_shipped_checkpoints_load():
-    import glob
+    """The reference's shipped checkpoints (model_gin/*.pth, model_architecture/{gcn,gat,graphsage}_*.pth) load into the drop-in
+    modules key for key: their state_dict key names, dtypes and shapes are recorded in tests/golden/checkpoint_keys.json."""
+    import json
     chem = importlib.import_module("pretrain-gnns_b200.chem.model")
     bio = importlib.import_module("pretrain-gnns_b200.bio.model")
+    with open(os.path.join(os.path.dirname(__file__), "golden", "checkpoint_keys.json")) as fh:
+        rec = json.load(fh)   # {"files": {path: schema index}, "schemas": [{key: [dtype, shape]}]}
     n = 0
-    for mod, dom in ((chem, "chem"), (bio, "bio")):
-        for f in sorted(glob.glob(f"/root/reference/{dom}/model_gin/*.pth")):
-            sd = torch.load(f, map_location="cpu", weights_only=True)
-            assert str(mod.GNN(5, 300).load_state_dict(sd)) == "<All keys matched successfully>"
-            n += 1
-        for f in sorted(glob.glob(f"/root/reference/{dom}/model_architecture/*.pth")):
-            t = "gcn" if "gcn" in f else "gat" if "gat" in f else "graphsage" if "graphsage" in f else None
-            if t is None:
-                continue
-            sd = torch.load(f, map_location="cpu", weights_only=True)
-            assert str(mod.GNN(5, 300, gnn_type=t).load_state_dict(sd)) == "<All keys matched successfully>", f
-            n += 1
+    for f, i in sorted(rec["files"].items()):
+        keys = rec["schemas"][i]
+        mod = chem if f.startswith("chem/") else bio
+        t = "gin" if "/model_gin/" in f else "gcn" if "gcn" in f else "gat" if "gat" in f else "graphsage"
+        sd = {k: torch.zeros(shape, dtype=getattr(torch, dt)) for k, (dt, shape) in keys.items()}
+        assert str(mod.GNN(5, 300, gnn_type=t).load_state_dict(sd)) == "<All keys matched successfully>", f
+        n += 1
     assert n >= 18
 
 
