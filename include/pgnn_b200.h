@@ -279,6 +279,28 @@ PGNN_API int64_t pgnn_chem_gin_workspace_bytes(int64_t N, int64_t E, int64_t L, 
 /* test aid: byte offsets in the workspace of z1 [L][N][2D] (post-ReLU hidden), z2 [L][N][D] (pre-BatchNorm), BatchNorm batch mean
  * [L][D] and invstd [L][D] after a training forward: lets a test recover the ReLU decisions the encoder took */
 PGNN_API int pgnn_chem_gin_debug_layout(int64_t N, int64_t E, int64_t L, int64_t D, int64_t* out4);
+/* test aids for the 3xTF32 wgmma GEMM (precision 1), reachable here with every operand layout, tile width and epilogue:
+ *   pgnn_debug_tc_gemm: C[m,n] = sum_r A(m,r) B(n,r), r < K.  a_kc / b_kc != 0: the operand is reduction-contiguous
+ *     (A(m,r) = A[m*lda + r]), else A(m,r) = A[r*lda + m] (same for B with n).  bn = the tile width, 64 or 128.  Epilogue as in
+ *     the encoders: + bias[N], relu != 0 (NaN kept), mask [M, ldm] (0 where mask <= 0 or NaN); then, all accumulated with
+ *     atomics into caller-zeroed buffers, colsum[N] += column sums, stats[2][N] += fp64 sums and sums of squares,
+ *     gT[q][n] (q < q_split) / gT2[q - q_split][n] (q >= q_split), row stride ldt, += sum_m S[m*Q + q] C[m,n] for 1 <= Q <= 16.
+ *     Optional pointers may be NULL.  PGNN_EUNSUPPORTED when lda or ldb is not a multiple of 4 or A / B is not 16-byte aligned.
+ *   pgnn_debug_tc_wgrad: gw[N,K] = gy[M,N]^T . x[M,K], gb[N] = column sums of gy (may be NULL), split-K over the M rows: with
+ *     partials (16-byte aligned, >= splits*N*K floats, N*K % 4 == 0) each split stores a partial tile and one kernel folds them
+ *     in split order; otherwise the splits accumulate with atomics.
+ *   pgnn_debug_tc_wgrad_plan: host only; out4 = {tile width, output tiles, splits, rows per split} of that GEMM.
+ *   pgnn_debug_transpose_batch: out[i] [cols[i], rows[i]] = transpose of in[i] [rows[i], cols[i]] for count <= 32 jobs (HOST arrays
+ *     of device pointers and sizes); PGNN_EUNSUPPORTED above 32. */
+PGNN_API int pgnn_debug_tc_gemm(int a_kc, int b_kc, int bn, const float* A, int64_t lda, const float* B, int64_t ldb, float* C,
+                                int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias, int relu, const float* mask,
+                                int64_t ldm, float* colsum, double* stats, const float* S, int Q, float* gT, float* gT2,
+                                int q_split, int64_t ldt, void* stream);
+PGNN_API int pgnn_debug_tc_wgrad(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K,
+                                 float* gw, float* gb, float* partials, int64_t partial_floats, void* stream);
+PGNN_API int pgnn_debug_tc_wgrad_plan(int64_t M, int64_t N, int64_t K, int64_t* out4);
+PGNN_API int pgnn_debug_transpose_batch(int count, const float* const* in, float* const* out, const int32_t* rows,
+                                        const int32_t* cols, void* stream);
 PGNN_API int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
                                    void* const* bn_num_batches_tracked, const int64_t* x, const int64_t* edge_index,
                                    const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, int training,

@@ -43,11 +43,12 @@ static inline int64_t align_up(int64_t a, int64_t b) { return ceil_div(a, b) * b
 
 // Optional column reductions fused into the tensor-core GEMM epilogue (the output tile is already staged in shared
 // memory there).  All outputs must be zeroed by the caller; every CTA adds its tile's contribution with atomics.
+constexpr int kMaxHookQ = 16;  // columns of S the epilogue holds per row (its shared-memory slice is [128][kMaxHookQ])
 struct PgnnGemmHooks {
   float* colsum = nullptr;   // [N]     += sum over rows of the (final) output              -> bias gradients
   double* stats = nullptr;   // [2][N]  += sum, sum of squares (fp64)                        -> BatchNorm batch statistics
   const float* S = nullptr;  // [M][Q]  per-row weights: gT[q][n] += sum_m S[m][q] out[m][n] -> bond-table gradients
-  int Q = 0;
+  int Q = 0;                 // 1 <= Q <= kMaxHookQ when S is set
   float* gT = nullptr;       // rows [0, q_split)
   float* gT2 = nullptr;      // rows [q_split, Q)
   int q_split = 0;
@@ -146,6 +147,9 @@ inline cudaError_t pgnn_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, 
   if (prof) pgnn_profile_mark(reinterpret_cast<const void*>(kernel), st, true);
   return err;
 }
+
+// max(v, 0) that keeps NaN, as torch.relu does (fmaxf(NaN, 0) would return 0 and hide a diverging value)
+__device__ __forceinline__ float relu_keep_nan(float v) { return v < 0.f ? 0.f : v; }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -142,7 +142,7 @@ k_sgemm(const float* __restrict__ A, int64_t lda, const float* __restrict__ B, i
       if (gn >= N) continue;
       float v = acc[i][j];
       if (ep.bias && blockIdx.z == 0) v += ep.bias[gn];
-      if (ep.relu) v = fmaxf(v, 0.f);
+      if (ep.relu) v = relu_keep_nan(v);
       if (ep.mask_src) v = (ep.mask_src[(int64_t)gm * ep.ldm + gn] > 0.f) ? v : 0.f;
       float* dst = Cout + (int64_t)gm * ldc + gn;
       if (ep.atomic) atomicAdd(dst, v); else *dst = v;

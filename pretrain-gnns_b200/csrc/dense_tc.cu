@@ -71,6 +71,19 @@ __device__ __forceinline__ void fence_acc(float (&d)[32]) {
 
 __device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
+// x = hi + lo with hi = trunc_tf32(x).  The add of +0 turns a NaN into a NaN with its payload in the high mantissa bits (the GPU's
+// canonical NaN), so that a payload only in the 13 truncated bits does not become Inf; finite values pass unchanged.  A non-finite
+// x has lo = NaN: see sum_chains.
+__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
+  hi = tf32_trunc(__fadd_rn(x, 0.f));
+  lo = x - hi;
+}
+
+// hi*hi chain + cross terms.  A non-finite operand makes the cross terms NaN (its lo part is NaN, or Inf meets an exact-zero lo),
+// while the hi*hi chain holds what the fp32 GEMM gives: every genuine fp32 NaN (a NaN input, Inf - Inf, Inf * 0) reaches that chain
+// as a NaN, so a +-Inf there is the fp32 result.
+__device__ __forceinline__ float sum_chains(float acc, float accx) { return isinf(acc) ? acc : acc + accx; }
+
 // Operand tile loader.  KC: source contiguous along the reduction (element (r,k) at src[r*ld + k]); otherwise contiguous
 // along the row index (element (r,k) at src[k*ld + r]).  R = rows (MN extent) of the tile.  Each thread owns NV 16-byte
 // pieces of a [R x BK] block.  MN-major pieces are assigned so that a warp covers 16 rows x 8 k: 64-byte global segments,
@@ -137,20 +150,24 @@ struct Loader {
     for (int i = 0; i < NV; ++i) {
       int rr, kk;
       piece(threadIdx.x + i * NTHREADS, rr, kk);
-      const float4 x = v[i];
-      const float4 h = make_float4(tf32_trunc(x.x), tf32_trunc(x.y), tf32_trunc(x.z), tf32_trunc(x.w));
-      const float4 l = make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
       if (KC) {
+        float4 h, l;
+        split_tf32(v[i].x, h.x, l.x);
+        split_tf32(v[i].y, h.y, l.y);
+        split_tf32(v[i].z, h.z, l.z);
+        split_tf32(v[i].w, h.w, l.w);
         const int o = sw128_off(rr, kk);
         *reinterpret_cast<float4*>(hi + o) = h;
         *reinterpret_cast<float4*>(lo + o) = l;
       } else {
-        const float hv[4] = {h.x, h.y, h.z, h.w}, lv[4] = {l.x, l.y, l.z, l.w};
+        const float xv[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
+          float h, l;
+          split_tf32(xv[q], h, l);
           const int o = sw128_off(rr + q, kk);
-          *reinterpret_cast<float*>(hi + o) = hv[q];
-          *reinterpret_cast<float*>(lo + o) = lv[q];
+          *reinterpret_cast<float*>(hi + o) = h;
+          *reinterpret_cast<float*>(lo + o) = l;
         }
       }
     }
@@ -163,7 +180,7 @@ struct TileCfg {
   static constexpr int B_BYTES = BN * BK * 4;
   static constexpr int STAGE = 2 * (A_BYTES + B_BYTES);  // [A hi | A lo | B hi | B lo]
   static constexpr int SLD = BN + 4;                     // epilogue staging row stride (16-byte aligned rows)
-  static constexpr int EPI = BM * SLD * 4 + BM * 16 * 4;  // staging tile + the hooks' [128][Q <= 16] slice
+  static constexpr int EPI = BM * SLD * 4 + BM * kMaxHookQ * 4;  // staging tile + the hooks' [128][Q <= 16] slice
   static constexpr int RING = 2 * STAGE;
   static constexpr int SMEM = (RING > EPI ? RING : EPI) + 1024;  // + alignment slack of the 1024-byte swizzle atoms
   // two CTAs per SM at BN = 64 (96 KiB of stages, <= 128 registers), one at BN = 128
@@ -219,7 +236,7 @@ __device__ __forceinline__ void tile_epilogue(float* stage, const float* s_bias,
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         if (s_bias_on) ov[q] += bv[q];
-        if (ep.relu) ov[q] = fmaxf(ov[q], 0.f);
+        if (ep.relu) ov[q] = relu_keep_nan(ov[q]);
         ov[q] = mv[q] > 0.f ? ov[q] : 0.f;
       }
       if (want_hooks)  // keep the final values in the staging tile for the column reductions below
@@ -249,16 +266,16 @@ __device__ __forceinline__ void tile_epilogue(float* stage, const float* s_bias,
       const int Q = ep.hooks.Q;
       float s1 = 0.f;
       double d1 = 0.0, d2 = 0.0;
-      float tq[16];
+      float tq[kMaxHookQ];
 #pragma unroll
-      for (int q = 0; q < 16; ++q) tq[q] = 0.f;
+      for (int q = 0; q < kMaxHookQ; ++q) tq[q] = 0.f;
       for (int r = 0; r < rows_here; ++r) {
         const float v = stage[r * SLD + c];
         s1 += v;
         if (ep.hooks.stats) { d1 += (double)v; d2 += (double)v * (double)v; }
         if (ep.hooks.S) {
 #pragma unroll
-          for (int q = 0; q < 16; ++q)
+          for (int q = 0; q < kMaxHookQ; ++q)
             if (q < Q) tq[q] = fmaf(sS[r * Q + q], v, tq[q]);
         }
       }
@@ -269,7 +286,7 @@ __device__ __forceinline__ void tile_epilogue(float* stage, const float* s_bias,
       }
       if (ep.hooks.S) {
 #pragma unroll
-        for (int q = 0; q < 16; ++q)
+        for (int q = 0; q < kMaxHookQ; ++q)
           if (q < Q)
             atomicAdd(q < ep.hooks.q_split ? &ep.hooks.gT[(int64_t)q * ep.hooks.ldt + n0 + c]
                                            : &ep.hooks.gT2[(int64_t)(q - ep.hooks.q_split) * ep.hooks.ldt + n0 + c], tq[q]);
@@ -371,9 +388,9 @@ k_gemm_3xtf32(const float* __restrict__ A, int64_t lda, const float* __restrict_
       for (int i = 0; i < 8; ++i) {
         const int col = h * 64 + i * 8 + (lane & 3) * 2;
         *reinterpret_cast<float2*>(stage + row * Cfg::SLD + col) =
-            make_float2(acc[h][4 * i] + accx[h][4 * i], acc[h][4 * i + 1] + accx[h][4 * i + 1]);
+            make_float2(sum_chains(acc[h][4 * i], accx[h][4 * i]), sum_chains(acc[h][4 * i + 1], accx[h][4 * i + 1]));
         *reinterpret_cast<float2*>(stage + (row + 8) * Cfg::SLD + col) =
-            make_float2(acc[h][4 * i + 2] + accx[h][4 * i + 2], acc[h][4 * i + 3] + accx[h][4 * i + 3]);
+            make_float2(sum_chains(acc[h][4 * i + 2], accx[h][4 * i + 2]), sum_chains(acc[h][4 * i + 3], accx[h][4 * i + 3]));
       }
   }
   __syncthreads();
@@ -409,10 +426,14 @@ template <bool A_KC, bool B_KC, int BN>
 int launch(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N, int K, int splits,
            int k_per_split, const TcEpilogue& ep, cudaStream_t st) {
   constexpr int smem = TileCfg<BN>::SMEM;
-  static bool configured = false;
-  if (!configured) {
+  // the shared-memory opt-in belongs to the current device's context: set it once per device (bit d = device d)
+  static std::atomic<uint64_t> configured{0};
+  int dev = 0;
+  PGNN_CUDA(cudaGetDevice(&dev));
+  const uint64_t bit = dev < 64 ? (uint64_t)1 << dev : 0;
+  if (!(configured.load(std::memory_order_relaxed) & bit)) {
     PGNN_CUDA(cudaFuncSetAttribute(k_gemm_3xtf32<A_KC, B_KC, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    configured = true;
+    configured.fetch_or(bit, std::memory_order_relaxed);
   }
   dim3 grid((unsigned)ceil_div(N, BN), (unsigned)ceil_div(M, BM), (unsigned)splits);
   PGNN_CUDA(pgnn_launch(k_gemm_3xtf32<A_KC, B_KC, BN>, dim3(grid), dim3(NTHREADS), smem, st, A, lda, B, ldb, C, ldc, M, N, K, k_per_split, ep));
@@ -432,23 +453,41 @@ inline int pick_bn(int M, int N, int splits) {
 template <bool A_KC, bool B_KC>
 int dispatch(int bn, const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N, int K, int splits,
              int k_per_split, const TcEpilogue& ep, cudaStream_t st) {
+  if (ep.hooks.S && (ep.hooks.Q < 1 || ep.hooks.Q > kMaxHookQ)) return PGNN_EINVAL;
   if (bn == 64) return launch<A_KC, B_KC, 64>(A, lda, B, ldb, C, ldc, M, N, K, splits, k_per_split, ep, st);
   return launch<A_KC, B_KC, 128>(A, lda, B, ldb, C, ldc, M, N, K, splits, k_per_split, ep, st);
 }
 
 }  // namespace
 
-// development entry: C[M,N] = sum_r A(m,r) B(n,r) with explicit operand majors (1 = reduction-contiguous)
-extern "C" __attribute__((visibility("default"))) int pgnn_debug_tc_gemm(int a_kc, int b_kc, int bn, const float* A, int64_t lda,
-                                                                        const float* B, int64_t ldb, float* C, int64_t ldc, int M,
-                                                                        int N, int K, void* stream) {
-  TcEpilogue ep{nullptr, 0, nullptr, 0, 0, PgnnGemmHooks{}};
-  cudaStream_t st = as_stream(stream);
+extern "C" int pgnn_debug_tc_gemm(int a_kc, int b_kc, int bn, const float* A, int64_t lda, const float* B, int64_t ldb, float* C,
+                                  int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias, int relu, const float* mask,
+                                  int64_t ldm, float* colsum, double* stats, const float* S, int Q, float* gT, float* gT2,
+                                  int q_split, int64_t ldt, void* stream) {
+  PGNN_CHECK_ARG(bn == 64 || bn == 128);
+  PGNN_CHECK_ARG(M > 0 && N > 0 && K > 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31));
+  PGNN_CHECK_ARG(A && B && C && ldc >= N && lda >= (a_kc ? K : M) && ldb >= (b_kc ? K : N));
+  PGNN_CHECK_ARG(!mask || ldm >= N);
+  if (S) {
+    PGNN_CHECK_ARG(Q >= 1 && Q <= kMaxHookQ && q_split >= 0 && q_split <= Q && ldt >= N);
+    PGNN_CHECK_ARG((q_split == 0 || gT) && (q_split == Q || gT2));
+  }
   if (lda % 4 || ldb % 4 || !aligned16(A) || !aligned16(B)) return PGNN_EUNSUPPORTED;
-  if (a_kc && b_kc) return dispatch<true, true>(bn, A, lda, B, ldb, C, ldc, M, N, K, 1, K, ep, st);
-  if (a_kc && !b_kc) return dispatch<true, false>(bn, A, lda, B, ldb, C, ldc, M, N, K, 1, K, ep, st);
-  if (!a_kc && b_kc) return dispatch<false, true>(bn, A, lda, B, ldb, C, ldc, M, N, K, 1, K, ep, st);
-  return dispatch<false, false>(bn, A, lda, B, ldb, C, ldc, M, N, K, 1, K, ep, st);
+  TcEpilogue ep{bias, relu, mask, ldm, 0, PgnnGemmHooks{}};
+  ep.hooks.colsum = colsum;
+  ep.hooks.stats = stats;
+  ep.hooks.S = S;
+  ep.hooks.Q = S ? Q : 0;
+  ep.hooks.gT = gT;
+  ep.hooks.gT2 = gT2;
+  ep.hooks.q_split = q_split;
+  ep.hooks.ldt = ldt;
+  cudaStream_t st = as_stream(stream);
+  const int m = (int)M, n = (int)N, k = (int)K;
+  if (a_kc && b_kc) return dispatch<true, true>(bn, A, lda, B, ldb, C, ldc, m, n, k, 1, k, ep, st);
+  if (a_kc && !b_kc) return dispatch<true, false>(bn, A, lda, B, ldb, C, ldc, m, n, k, 1, k, ep, st);
+  if (!a_kc && b_kc) return dispatch<false, true>(bn, A, lda, B, ldb, C, ldc, m, n, k, 1, k, ep, st);
+  return dispatch<false, false>(bn, A, lda, B, ldb, C, ldc, m, n, k, 1, k, ep, st);
 }
 
 // y[M,N] = act(x[M,K] . w[N,K]^T + bias)
@@ -574,7 +613,7 @@ int pgnn_tc_linear_bwd_w_ws(const float* gy, int64_t ldgy, const float* x, int64
   const WgradPlan plan = wgrad_plan(M, N, K);
   const int bn = plan.bn, splits = plan.splits, per = plan.per;
   int rc;
-  if (splits > 1 && partials && partial_floats >= (int64_t)splits * N * K && ((N * K) % 4 == 0)) {
+  if (splits > 1 && partials && aligned16(partials) && partial_floats >= (int64_t)splits * N * K && ((N * K) % 4 == 0)) {
     // split s writes its tile into partials[s] (the kernel offsets C by blockIdx.z * ep.split_stride)
     TcEpilogue ep{nullptr, 0, nullptr, 0, 0, PgnnGemmHooks{}};
     ep.split_stride = N * K;
@@ -605,3 +644,36 @@ int pgnn_tc_linear_bwd_w(const float* gy, int64_t ldgy, const float* x, int64_t 
                          float* gb, cudaStream_t st) {
   return pgnn_tc_linear_bwd_w_ws(gy, ldgy, x, ldx, M, N, K, gw, gb, nullptr, 0, st);
 }
+
+// test entry points (include/pgnn_b200.h): the weight-gradient GEMM with a caller-chosen split-K workspace, its plan, and the
+// weight-transpose batch of the encoder backward
+extern "C" {
+
+int pgnn_debug_tc_wgrad(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
+                        float* gb, float* partials, int64_t partial_floats, void* stream) {
+  PGNN_CHECK_ARG(M > 0 && N > 0 && K > 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31));
+  PGNN_CHECK_ARG(gy && x && gw && ldgy >= N && ldx >= K && partial_floats >= 0);
+  return pgnn_tc_linear_bwd_w_ws(gy, ldgy, x, ldx, M, N, K, gw, gb, partials, partial_floats, as_stream(stream));
+}
+
+int pgnn_debug_tc_wgrad_plan(int64_t M, int64_t N, int64_t K, int64_t* out4) {
+  PGNN_CHECK_ARG(M > 0 && N > 0 && K > 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31) && out4);
+  const WgradPlan p = wgrad_plan(M, N, K);
+  out4[0] = p.bn;
+  out4[1] = p.tiles;
+  out4[2] = p.splits;
+  out4[3] = p.per;
+  return PGNN_OK;
+}
+
+int pgnn_debug_transpose_batch(int count, const float* const* in, float* const* out, const int32_t* rows, const int32_t* cols,
+                               void* stream) {
+  PGNN_CHECK_ARG(count >= 0);
+  if (count == 0) return PGNN_OK;
+  PGNN_CHECK_ARG(in && out && rows && cols);
+  if (count > kMaxTransposeJobs) return PGNN_EUNSUPPORTED;
+  for (int i = 0; i < count; ++i) PGNN_CHECK_ARG(in[i] && out[i] && rows[i] > 0 && cols[i] > 0);
+  return pgnn_internal_transpose_batch(count, in, out, rows, cols, as_stream(stream));
+}
+
+}  // extern "C"

@@ -952,7 +952,7 @@ class _MaskedCE(Function):
         if idx.dtype != torch.int64 or labels.dtype != torch.int64 or (idx2 is not None and idx2.dtype != torch.int64):
             raise PgnnError("indices and labels must be int64")
         M, D, V = idx.shape[0], rep.shape[1], w.shape[0]
-        ldv = _pad4(V)  # 16-byte aligned logit rows: the TMA boxes of the backward GEMMs zero-fill the ragged class extent
+        ldv = _pad4(V)  # 16-byte aligned logit rows (the tensor path's vector loads); the GEMM loaders never read past column V
         dev = rep.device
         rows = torch.empty(M, D, dtype=torch.float32, device=dev)
         check(lib.pgnn_row_gather_fwd(_p(rep), rep.stride(0), rep.shape[0], _p(idx), _p(idx2), M, D, _p(rows), D, _st()), "row_gather_fwd")
