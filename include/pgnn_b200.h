@@ -128,7 +128,7 @@ PGNN_API int pgnn_bio_embed_bwd(const float* x, const float* g, int64_t ldg, int
  *                                                                              bio/model.py:54-55)
  * x may be given as (pre-BN activations, per-column affine, ReLU flag): x_eff = act(x * in_scale + in_shift)
  * so a BatchNorm + ReLU (chem/model.py:269-275) is applied on load instead of in a pass of its own
- * (in_scale == NULL -> identity).
+ * (in_scale == NULL -> identity).  The ReLU keeps NaN, as torch.relu does.
  * ------------------------------------------------------------------------------------------- */
 PGNN_API int pgnn_aggregate_fwd(const float* x, int64_t ldx, const float* in_scale, const float* in_shift,
                                 int in_relu, int64_t num_nodes, int64_t C,
@@ -185,7 +185,8 @@ PGNN_API int pgnn_bn_bwd(const float* gy, int64_t ldgy, const float* x, int64_t 
                          const float* gamma, const float* beta, const float* save_mean,
                          const float* save_invstd, int relu, float* gx, int64_t ldgx, float* ggamma,
                          float* gbeta, void* workspace, int64_t workspace_bytes, void* stream);
-/* y = relu(x), gx = gy * (y > 0): the inter-layer ReLU of bio/model.py:281 (no BatchNorm there) */
+/* y = relu(x), gx = gy * (y > 0): the inter-layer ReLU of bio/model.py:281 (no BatchNorm there).  relu keeps NaN, as
+ * torch.relu does, here and in the BatchNorm entry points above. */
 PGNN_API int pgnn_relu_fwd(const float* x, int64_t ldx, int64_t M, int64_t C, float* y, int64_t ldy, void* stream);
 PGNN_API int pgnn_relu_bwd(const float* gy, int64_t ldgy, const float* y, int64_t ldy_, int64_t M, int64_t C,
                            float* gx, int64_t ldgx, void* stream);

@@ -26,10 +26,10 @@ __device__ __forceinline__ float4 affine_act(float4 v, const float* __restrict__
     v.w = fmaf(v.w, a.w, b.w);
   }
   if (relu) {
-    v.x = fmaxf(v.x, 0.f);
-    v.y = fmaxf(v.y, 0.f);
-    v.z = fmaxf(v.z, 0.f);
-    v.w = fmaxf(v.w, 0.f);
+    v.x = relu_keep_nan(v.x);
+    v.y = relu_keep_nan(v.y);
+    v.z = relu_keep_nan(v.z);
+    v.w = relu_keep_nan(v.w);
   }
   return v;
 }

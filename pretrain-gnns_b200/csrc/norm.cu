@@ -101,7 +101,7 @@ k_bn_apply(const float* __restrict__ x, int64_t ldx, int64_t M, int C, const flo
     const int64_t r = idx / C;
     const int c = (int)(idx - r * C);
     float v = fmaf((x[r * ldx + c] - mean[c]) * invstd[c], gamma[c], beta[c]);
-    if (relu) v = fmaxf(v, 0.f);
+    if (relu) v = relu_keep_nan(v);
     y[r * ldy + c] = v;
   }
 }
@@ -119,7 +119,7 @@ k_bn_apply_fold(const float* __restrict__ x, int64_t ldx, int64_t M, int C, Pgnn
     const int64_t r = idx / C;
     const int c = (int)(idx - r * C);
     float v = fmaf(x[r * ldx + c], s_aff[c], s_aff[C + c]);
-    if (relu) v = fmaxf(v, 0.f);
+    if (relu) v = relu_keep_nan(v);
     y[r * ldy + c] = v;
   }
 }
@@ -135,7 +135,7 @@ k_bn_eval(const float* __restrict__ x, int64_t ldx, int64_t M, int C, const floa
     const int c = (int)(idx - r * C);
     const float invstd = __frcp_rn(__fsqrt_rn(rv[c] + eps));
     float v = fmaf((x[r * ldx + c] - rm[c]) * invstd, gamma[c], beta[c]);
-    if (relu) v = fmaxf(v, 0.f);
+    if (relu) v = relu_keep_nan(v);
     y[r * ldy + c] = v;
   }
 }
@@ -380,7 +380,7 @@ k_bn_apply_v4(const float* __restrict__ x, int64_t ldx, int64_t M, int C4, const
     o.z = fmaf((xv.z - mu.z) * is.z, ga.z, be.z);
     o.w = fmaf((xv.w - mu.w) * is.w, ga.w, be.w);
     if (relu) {
-      o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
+      o.x = relu_keep_nan(o.x); o.y = relu_keep_nan(o.y); o.z = relu_keep_nan(o.z); o.w = relu_keep_nan(o.w);
     }
     *reinterpret_cast<float4*>(y + r * ldy + c) = o;
   }
@@ -393,7 +393,7 @@ k_relu_fwd(const float* __restrict__ x, int64_t ldx, int64_t M, int C, float* __
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = idx / C;
     const int c = (int)(idx - r * C);
-    y[r * ldy + c] = fmaxf(x[r * ldx + c], 0.f);
+    y[r * ldy + c] = relu_keep_nan(x[r * ldx + c]);
   }
 }
 __global__ void __launch_bounds__(256)
@@ -418,7 +418,7 @@ k_relu_fwd_v4(const float* __restrict__ x, int64_t ldx, int64_t M, int C4, float
     const int64_t r = idx / C4;
     const int c = (int)(idx - r * C4) * 4;
     const float4 v = *reinterpret_cast<const float4*>(x + r * ldx + c);
-    *reinterpret_cast<float4*>(y + r * ldy + c) = make_float4(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f), fmaxf(v.z, 0.f), fmaxf(v.w, 0.f));
+    *reinterpret_cast<float4*>(y + r * ldy + c) = make_float4(relu_keep_nan(v.x), relu_keep_nan(v.y), relu_keep_nan(v.z), relu_keep_nan(v.w));
   }
 }
 __global__ void __launch_bounds__(256)

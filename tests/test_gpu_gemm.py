@@ -23,11 +23,11 @@ import numpy as np
 import pytest
 import torch
 
+from device_buffers import DEV, NAN, SENT, Region, ceil4 as _ceil4, card as _card, operand, zeroed
 from golden_util import write_report
 
 cabi = importlib.import_module("pretrain-gnns_b200._cabi")
 gpu = pytest.mark.gpu
-DEV = "cuda:0"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OK, EINVAL, EUNSUPPORTED = 0, -1, -4
 LAYOUTS = ((1, 1), (1, 0), (0, 1), (0, 0))  # (A reduction-contiguous, B reduction-contiguous)
@@ -36,53 +36,10 @@ COMBOS = [(ak, bk, bn) for ak, bk in LAYOUTS for bn in (64, 128)]
 # fp32 GEMM <= 2e-7, one cross term dropped >= 1.1e-4, plain TF32 >= 2e-4.  Measured on an H100 80GB HBM3 at 700 W: <= 6.2e-7 for
 # K <= 600, 1.24e-6 for the 5986-long reduction, in every layout and tile width (DESIGN.md §4).
 TAU = 5e-6
-SENT = -7777.25  # output sentinel
-NAN = float("nan")
 
 
 def _stream():
     return torch.cuda.current_stream().cuda_stream
-
-
-def _ceil4(n):
-    return (n + 3) // 4 * 4
-
-
-class Region:
-    """A [rows, cols] view with row stride ld inside a device allocation filled with `fill`: columns past cols, two rows past
-    the view and some slack after them hold `fill`; `shift` floats precede the view."""
-
-    def __init__(self, rows, cols, ld, fill, shift=0, dtype=torch.float32):
-        self.shape, self.fill = (rows, cols, ld, shift), fill
-        self.buf = torch.full((shift + (rows + 2) * ld + 7,), fill, dtype=dtype, device=DEV)
-        self.view = self._view(self.buf)
-        self.ld = ld
-
-    def _view(self, buf):
-        rows, cols, ld, shift = self.shape
-        return buf[shift:shift + rows * ld].view(rows, ld)[:, :cols]
-
-    def ptr(self):
-        return self.view.data_ptr()
-
-    def outside_intact(self):
-        c = self.buf.clone()
-        self._view(c).fill_(self.fill)
-        return bool((c == self.fill).all())
-
-
-def operand(t, kc, pad=4, shift=0):
-    """Logical [R, K] operand (CPU fp32) stored reduction-contiguous (kc) or as its transpose, in a NaN-poisoned region."""
-    s = t if kc else t.t()
-    r = Region(s.shape[0], s.shape[1], _ceil4(s.shape[1]) + pad, NAN, shift=shift)
-    r.view.copy_(s)
-    return r
-
-
-def zeroed(rows, cols, ld, dtype=torch.float32):
-    r = Region(rows, cols, ld, SENT, dtype=dtype)
-    r.view.zero_()
-    return r
 
 
 def tc_gemm(a, b, a_kc, b_kc, bn, bias=None, relu=False, mask=None, ldm_pad=4, mask_shift=0, colsum=False, stats=False, S=None,
@@ -169,16 +126,6 @@ def exact_ref(a, b, **ep):
 
 def rnd(*shape, seed=0):
     return torch.randn(*shape, generator=torch.Generator().manual_seed(seed))
-
-
-def _card():
-    name = torch.cuda.get_device_name(0)
-    try:
-        pl = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                            text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        pl = "unknown"
-    return dict(card=name, power_limit=pl)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -548,12 +495,13 @@ _TWO_DEVICES = textwrap.dedent("""
     import sys
     sys.path.insert(0, sys.argv[1]); sys.path.insert(0, sys.argv[1] + "/tests")
     import torch
+    import device_buffers as B
     import test_gpu_gemm as T
     a, b = T.rnd(300, 600, seed=1), T.rnd(190, 600, seed=2)
     ref, den = T.reference(a, b), T.scale_of(a, b)
     for d in (0, 1):
         torch.cuda.set_device(d)
-        T.DEV = "cuda:%d" % d
+        B.DEV = T.DEV = "cuda:%d" % d
         for ak, bk, bn in T.COMBOS:
             e = T.norm_err(T.tc_gemm(a, b, ak, bk, bn)["C"], ref, den)
             assert e <= T.TAU, (d, ak, bk, bn, e)
