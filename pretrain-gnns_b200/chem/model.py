@@ -12,8 +12,6 @@ and the same parameter / buffer names, so every shipped `.pth` loads with all ke
 is underneath: no torch_geometric, no per-edge tensors.  Each batch is bucketed once (ops.Graph), the bond
 embedding sum is folded into a per-node 9-bin summary, and every op is a CUDA kernel behind the C ABI.
 """
-import os
-
 import torch
 import torch.nn.functional as F
 from torch import nn
@@ -149,7 +147,7 @@ class GNN(nn.Module):
         self.gnns = nn.ModuleList([_CONVS[gnn_type](emb_dim) for _ in range(num_layer)])
         self.batch_norms = nn.ModuleList([nn.BatchNorm1d(emb_dim) for _ in range(num_layer)])
         self._gnn_type = gnn_type
-        self._plan = None          # lazily built bookkeeping of the fused GIN path (ops.ChemGinPlan)
+        self._plan = None          # lazily built bookkeeping of the whole-encoder path (ops.ChemEncoderPlan)
         self.fused = True          # set False to force the layer-by-layer composition (used by the tests)
 
     _DEFAULT_AGGR = {"gin": "add", "gcn": "add", "gat": "add", "graphsage": "mean"}
@@ -159,14 +157,12 @@ class GNN(nn.Module):
         default aggregation (and GAT's 2 heads / slope 0.2) and no live dropout."""
         if not (self.fused and self.JK == "last" and (self.drop_ratio == 0 or not self.training)):
             return None
-        if self._gnn_type != "gin" and os.environ.get("PGNN_FUSED_CONV", "1") == "0":   # development switch
-            return None
         if any(conv.aggr != self._DEFAULT_AGGR[self._gnn_type] for conv in self.gnns) or any(bn.training != self.training for bn in self.batch_norms):
             return None
         if self._gnn_type == "gat" and any(conv.heads != 2 or conv.negative_slope != 0.2 for conv in self.gnns):
             return None
         if self._plan is None:
-            self._plan = ops.ChemGinPlan(self) if self._gnn_type == "gin" else ops.ChemConvPlan(self, self._gnn_type)
+            self._plan = ops.ChemEncoderPlan(self, self._gnn_type)
         return self._plan
 
     def forward(self, *argv):
@@ -178,8 +174,7 @@ class GNN(nn.Module):
             raise ValueError("unmatched number of arguments.")
         plan = self._fused_plan()
         if plan is not None:
-            enc = ops.chem_gin_encoder if self._gnn_type == "gin" else ops.chem_conv_encoder
-            return enc(plan, x, edge_index, edge_attr, self.training)
+            return ops.chem_encoder(plan, x, edge_index, edge_attr, self.training)
         graph = ops.graph_for(edge_index, x.size(0))
         h = ops.chem_embed(x, self.x_embedding1.weight, self.x_embedding2.weight)
         hs = [h]

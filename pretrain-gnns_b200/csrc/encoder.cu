@@ -1,13 +1,21 @@
-// Whole-encoder entry points for the chem GIN stack (chem/model.py:255-290 with gnn_type="gin", JK="last",
-// drop_ratio=0): ONE call enqueues graph preparation, the atom embedding and all L x (aggregate -> MLP ->
-// BatchNorm[-> ReLU]) layers; a second call enqueues the whole backward.  This is what GNN.forward binds
-// to, so a training step crosses the Python/C boundary twice instead of ~60 times, and the inter-layer
-// BatchNorm + ReLU never makes a pass of its own: layer l only accumulates the batch statistics and layer
-// l+1's gather applies scale/shift/ReLU while it loads the rows (pgnn_aggregate_fwd's in_scale/in_shift).
+// Whole-encoder entry points for the chem GNN (chem/model.py:206-290 with JK="last", drop_ratio=0): ONE call enqueues graph
+// preparation, the atom embedding and all L layers; a second call enqueues the whole backward.  This is what GNN.forward binds
+// to, so a training step crosses the Python/C boundary twice instead of ~60 (GIN) or ~100 (conv types) times, without the
+// per-op allocations and the torch.cat of the two bond tables per layer and pass.
 //
-// Parameters arrive as a host array of device pointers in a fixed order (PGNN_CHEM_GIN_* below), gradients
-// leave in ONE flat fp32 buffer with the library-defined layout of pgnn_chem_gin_grad_offsets, which is
-// also the buffer the data-parallel all-reduce runs on.
+//   GIN        (pgnn_chem_gin_*, chem/model.py:37-55):  L x (aggregate -> MLP -> BatchNorm[-> ReLU]).  The inter-layer
+//              BatchNorm + ReLU never makes a pass of its own: layer l only accumulates the batch statistics and layer l+1's
+//              gather applies scale/shift/ReLU while it loads the rows (pgnn_aggregate_fwd's in_scale/in_shift).
+//   pgnn_chem_conv_* with conv_type =
+//   GCN        (chem/model.py:85-104):   xl = Linear(D,D)(h);  out_i = sum_j d_i^-1/2 d_j^-1/2 (xl_j + e_ij)
+//   GraphSAGE  (chem/model.py:182-202):  xl = Linear(D,D)(h);  out_i = normalize(mean_j (xl_j + e_ij))
+//   GAT        (chem/model.py:134-165):  xl = Linear(D,2D)(h); out_i = mean_heads(sum_j alpha_ij (xl_j + e_ij)) + bias
+//   each followed by BatchNorm1d(D) and, except after the last layer, ReLU (chem/model.py:267-276).  The per-layer arithmetic
+//   is the operator-level C ABI of include/pgnn_b200.h (the same kernels the layer-by-layer Python composition launches).
+//
+// Parameters arrive as a host array of device pointers in a fixed order, gradients leave in ONE flat fp32 buffer with the
+// library-defined layout of pgnn_chem_gin_grad_offsets / pgnn_chem_conv_grad_offsets (grad_layout below), which is also the
+// buffer the data-parallel all-reduce runs on.
 #include "common.cuh"
 
 #include <cstdlib>
@@ -43,52 +51,120 @@ int pgnn_internal_bn_bwd_colsum(const float* gy, int64_t ldgy, const float* x, i
 
 namespace {
 
-// order of the parameter pointer table and of the flat gradient layout
-enum { P_XEMB1 = 0, P_XEMB2 = 1, P_LAYER0 = 2 };
-enum { L_W1 = 0, L_B1, L_W2, L_B2, L_ET1, L_ET2, L_GAMMA, L_BETA, L_COUNT };
-
+constexpr int kGin = 0;            // GIN's type code inside this file; the conv types use PGNN_CONV_* (never 0)
 constexpr int kAtomRows = 120, kChiralRows = 3;   // chem/model.py:9-10
 constexpr int kOneHotLd = 124;                    // kAtomRows + kChiralRows padded to a multiple of 4
+constexpr int kHeads = 2;          // chem/model.py:108 (heads=2 is what GNN.__init__ builds, :243)
+constexpr float kSlope = 0.2f;     // negative_slope, chem/model.py:108
 
+// order of the parameter pointer table and of the flat gradient layout
+enum { P_XEMB1 = 0, P_XEMB2 = 1, P_LAYER0 = 2 };
+// per-layer parameter order; the two bond tables are adjacent so that one [9, C] block holds both
+enum { L_W1 = 0, L_B1, L_W2, L_B2, L_ET1, L_ET2, L_GAMMA, L_BETA, L_COUNT };     // gin
+enum { G_W = 0, G_B, G_ET1, G_ET2, G_GAMMA, G_BETA, G_COUNT };                    // gcn / graphsage
+enum { A_W = 0, A_B, A_ATT, A_BIAS, A_ET1, A_ET2, A_GAMMA, A_BETA, A_COUNT };     // gat
+
+inline int layer_params(int type) { return type == kGin ? L_COUNT : type == PGNN_CONV_GAT ? A_COUNT : G_COUNT; }
+inline int agg_mode(int type) { return type == kGin ? PGNN_AGG_SUM : type == PGNN_CONV_GCN ? PGNN_AGG_GCN : PGNN_AGG_MEAN; }
+bool valid_conv(int t) { return t == PGNN_CONV_GCN || t == PGNN_CONV_SAGE || t == PGNN_CONV_GAT; }
+
+#define TRY(call)                     \
+  do {                                \
+    int rc__ = (call);                \
+    if (rc__ != PGNN_OK) return rc__; \
+  } while (0)
+
+// The flat gradient layout of one type: fills offsets[0..count] when given and returns the parameter count.
+int64_t grad_layout(int type, int64_t L, int64_t D, int64_t* offsets) {
+  if (!offsets) return 2 + (int64_t)layer_params(type) * L;
+  const int64_t HD = type == PGNN_CONV_GAT ? kHeads * D : D;
+  int64_t o = 0, i = 0;
+  auto next = [&](int64_t size) { offsets[i++] = o; o += size; };
+  next(kAtomRows * D);    // x_embedding1.weight
+  next(kChiralRows * D);  // x_embedding2.weight
+  for (int64_t l = 0; l < L; ++l) {
+    if (type == kGin) {
+      next(2 * D * D);  // mlp.0.weight [2D, D]
+      next(2 * D);      // mlp.0.bias
+      next(2 * D * D);  // mlp.2.weight [D, 2D]
+      next(D);          // mlp.2.bias
+    } else {
+      next(HD * D);     // linear.weight / weight_linear.weight [HD, D]
+      next(HD);         // its bias
+      if (type == PGNN_CONV_GAT) {
+        next(kHeads * 2 * D);  // att [1, H, 2D]
+        next(D);               // bias [D]
+      }
+    }
+    next(6 * HD);  // edge_embedding1.weight
+    next(3 * HD);  // edge_embedding2.weight
+    next(D);       // batch_norms.l.weight
+    next(D);       // batch_norms.l.bias
+  }
+  offsets[i] = o;
+  return i;
+}
+
+// 256-byte aligned regions of one workspace (base == nullptr only measures).  With `pad_empty` an empty region still takes one
+// element, as every conv region does; GIN's regions take no space when empty, except its edge arrays (carve_front).
 struct Carve {
   char* base;
+  bool pad_empty;
   int64_t off = 0;
-  explicit Carve(void* b) : base(reinterpret_cast<char*>(b)) {}
+  Carve(void* b, bool pad) : base(reinterpret_cast<char*>(b)), pad_empty(pad) {}
   template <typename T>
   T* take(int64_t count) {
     T* p = reinterpret_cast<T*>(base + off);
-    off += align_up(count * (int64_t)sizeof(T), 256);
+    off += align_up((pad_empty && count < 1 ? 1 : count) * (int64_t)sizeof(T), 256);
     return p;
   }
 };
 
-struct Ws {
+// the first regions of every type's workspace: what forward_prologue writes
+struct Front {
   int32_t *rowptr_t, *rowptr_s, *nbr_t, *eid_t, *nbr_s, *eid_s;
-  float *S, *h0, *scale, *shift, *mean, *invstd;  // scale/shift/mean/invstd: [L, D]
-  float* onehot;                                   // [N, kOneHotLd]: atom-code one-hot rows (embedding gradient as a GEMM)
-  double* bn_acc;                                  // [L][2][D] fp64 BatchNorm sums of the forward
-  float *aggr, *z1, *z2;                           // [L, N, D], [L, N, 2D], [L, N, D]
-  float *gh, *gz2, *gz1, *gaggr;                   // backward temporaries
-  float* wT;                                       // [L][2][2D*D]: mlp.0.weight^T, mlp.2.weight^T (dgrad B operands)
-  float* wpart;                                    // split-K partial tiles of one wgrad
+  float *S, *dinv, *h0;  // dinv: conv types only
+  float* onehot;         // [N, kOneHotLd]: atom-code one-hot rows (embedding gradient as a GEMM)
+};
+
+void carve_front(Carve& c, Front& f, int type, int64_t N, int64_t E, int64_t D) {
+  const int64_t e1 = E > 0 ? E : 1;
+  f.rowptr_t = c.take<int32_t>(N + 1);
+  f.rowptr_s = c.take<int32_t>(N + 1);
+  f.nbr_t = c.take<int32_t>(e1);
+  f.eid_t = c.take<int32_t>(e1);
+  f.nbr_s = c.take<int32_t>(e1);
+  f.eid_s = c.take<int32_t>(e1);
+  f.S = c.take<float>(N * 9);
+  f.dinv = type == kGin ? nullptr : c.take<float>(N);
+  f.h0 = c.take<float>(N * D);
+  f.onehot = c.take<float>(N * kOneHotLd);
+}
+
+// split-K partial tiles for the largest weight-gradient GEMM of a type: its layer wgrads ([N_out, D] with N_out = the given
+// width) and the embedding tables' gradient as a GEMM
+int64_t split_k_floats(int64_t N, int64_t width, int64_t D) {
+  const int64_t a = pgnn_tc_wgrad_workspace_floats(N, width, D);
+  const int64_t e = pgnn_tc_wgrad_workspace_floats(N, kAtomRows + kChiralRows, D);
+  return e > a ? e : a;
+}
+
+struct GinWs : Front {
+  float *scale, *shift, *mean, *invstd;  // [L, D]
+  double* bn_acc;                        // [L][2][D] fp64 BatchNorm sums of the forward
+  float *aggr, *z1, *z2;                 // [L, N, D], [L, N, 2D], [L, N, D]
+  float *gh, *gz2, *gz1, *gaggr;         // backward temporaries
+  float* wT;                             // [L][2][2D*D]: mlp.0.weight^T, mlp.2.weight^T (dgrad B operands)
+  float* wpart;                          // split-K partial tiles of one wgrad
   int64_t wpart_floats;
-  void* scratch;                                   // bucket / BatchNorm scratch
+  void* scratch;                         // bucket / BatchNorm scratch
   int64_t scratch_bytes, total;
 };
 
-Ws carve(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
-  Carve c(base);
-  Ws w;
-  const int64_t e1 = E > 0 ? E : 1;
-  w.rowptr_t = c.take<int32_t>(N + 1);
-  w.rowptr_s = c.take<int32_t>(N + 1);
-  w.nbr_t = c.take<int32_t>(e1);
-  w.eid_t = c.take<int32_t>(e1);
-  w.nbr_s = c.take<int32_t>(e1);
-  w.eid_s = c.take<int32_t>(e1);
-  w.S = c.take<float>(N * 9);
-  w.h0 = c.take<float>(N * D);
-  w.onehot = c.take<float>(N * kOneHotLd);
+GinWs carve_gin(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
+  Carve c(base, false);
+  GinWs w;
+  carve_front(c, w, kGin, N, E, D);
   w.bn_acc = c.take<double>(L * 2 * D);
   w.scale = c.take<float>(L * D);
   w.shift = c.take<float>(L * D);
@@ -102,11 +178,7 @@ Ws carve(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
   w.gz1 = c.take<float>(2 * N * 2 * D);   // them while layer l-1's backward writes the other copy
   w.gaggr = c.take<float>(N * D);
   w.wT = c.take<float>(L * 4 * D * D);
-  w.wpart_floats = pgnn_tc_wgrad_workspace_floats(N, 2 * D, D);  // both MLP weight gradients have 2D*D elements
-  {
-    const int64_t e = pgnn_tc_wgrad_workspace_floats(N, 123, D);  // the embedding tables' gradient as a GEMM
-    if (e > w.wpart_floats) w.wpart_floats = e;
-  }
+  w.wpart_floats = split_k_floats(N, 2 * D, D);  // both MLP weight gradients have 2D*D elements
   w.wpart = c.take<float>(w.wpart_floats);
   int64_t sb = pgnn_graph_prep_workspace_bytes(N, E);
   const int64_t bb = pgnn_bn_workspace_bytes(N > 0 ? N : 1, D);
@@ -117,14 +189,60 @@ Ws carve(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
   return w;
 }
 
-// Weight-gradient GEMMs on a side stream.  Per layer the critical path of the backward is BatchNorm-bwd -> dgrad2 -> dgrad1 ->
-// transpose gather -> (next layer); wgrad2 (needs gz2, z1) and wgrad1 (needs gz1, aggr) only feed the gradient buffer.  On
-// their own stream they run under the next layer's BatchNorm sweeps and gathers (LSU / L2-bound kernels that leave the tensor
-// pipe and most of shared memory idle) instead of in front of them.  Ordering is by events; gz2 / gz1 are double-buffered
-// by layer parity so the main stream never overwrites an operand a pending wgrad still reads.  PGNN_WGRAD_STREAM=0 disables.
+struct ConvWs : Front {
+  float *xl, *z, *hout;        // per layer: Linear output [N, HD], BatchNorm input [N, D], layer output [N, D]
+  float *nrm, *alpha, *pq, *T; // per layer: SAGE row norms [N]; GAT attention [(E+N), H], logit halves [N, H, 2], tables [9, HD]
+  float *mean, *invstd;        // [L, D]
+  float *gz, *ga, *gxl, *gh;   // backward temporaries [N, D], [N, D], [N, HD], [N, D]
+  float* wpart;
+  int64_t wpart_floats;
+  void* scratch;
+  int64_t scratch_bytes, total;
+};
+
+ConvWs carve_conv(void* base, int type, int64_t N, int64_t E, int64_t L, int64_t D) {
+  Carve c(base, true);
+  ConvWs w;
+  const int64_t HD = type == PGNN_CONV_GAT ? kHeads * D : D;
+  carve_front(c, w, type, N, E, D);
+  w.xl = c.take<float>(L * N * HD);
+  w.z = c.take<float>(L * N * D);
+  w.hout = c.take<float>(L * N * D);
+  w.nrm = c.take<float>(type == PGNN_CONV_SAGE ? L * N : 0);
+  w.alpha = c.take<float>(type == PGNN_CONV_GAT ? L * (E + N) * kHeads : 0);
+  w.pq = c.take<float>(type == PGNN_CONV_GAT ? L * N * kHeads * 2 : 0);
+  w.T = c.take<float>(type == PGNN_CONV_GAT ? L * 9 * HD : 0);
+  w.mean = c.take<float>(L * D);
+  w.invstd = c.take<float>(L * D);
+  w.gz = c.take<float>(N * D);
+  w.ga = c.take<float>(N * D);
+  w.gxl = c.take<float>(2 * N * HD);   // two copies by layer parity: the side-stream wgrad of layer l reads one while layer l-1 writes the other
+  w.gh = c.take<float>(N * D);
+  w.wpart_floats = split_k_floats(N, HD, D);
+  w.wpart = c.take<float>(w.wpart_floats);
+  int64_t sb = pgnn_graph_prep_workspace_bytes(N, E);
+  const int64_t bb = pgnn_bn_workspace_bytes(N > 0 ? N : 1, D);
+  if (bb > sb) sb = bb;
+  if (type == PGNN_CONV_GAT) {
+    const int64_t gb = pgnn_gat_bwd_workspace_bytes(N, E, kHeads, D);
+    if (gb > sb) sb = gb;
+  }
+  w.scratch_bytes = sb;
+  w.scratch = c.take<char>(sb);
+  w.total = c.off;
+  return w;
+}
+
+// Weight-gradient GEMMs on a side stream.  They only feed the gradient buffer (GIN: wgrad2 needs gz2, z1 and wgrad1 needs gz1,
+// aggr; conv types: one wgrad on gxl), so on their own stream they run under the next layer's BatchNorm sweeps, attention and
+// gathers (LSU / L2-bound kernels that leave the tensor pipe and most of shared memory idle) instead of in front of them.
+// Ordering is by events; the wgrad operands are double-buffered by layer parity so the main stream never overwrites an operand
+// a pending wgrad still reads.  ready[k][parity] / done[k][parity]: wgrad k's operand is written / wgrad k has finished (GIN
+// uses k = 0 for wgrad2, 1 for wgrad1; the conv types k = 0).  One context per (device, main stream) serves every type.
+// PGNN_WGRAD_STREAM=0 disables.
 struct SideCtx {
   cudaStream_t side = nullptr;
-  cudaEvent_t gz2_ready[2] = {}, gz1_ready[2] = {}, w2_done[2] = {}, w1_done[2] = {}, join = nullptr;
+  cudaEvent_t ready[2][2] = {}, done[2][2] = {}, join = nullptr;
   bool ok = false;
 };
 SideCtx* side_ctx(cudaStream_t main_stream) {
@@ -146,61 +264,69 @@ SideCtx* side_ctx(cudaStream_t main_stream) {
   SideCtx* c = new SideCtx();
   all[key] = c;
   bool ok = cudaStreamCreateWithFlags(&c->side, cudaStreamNonBlocking) == cudaSuccess;
-  for (int i = 0; i < 2 && ok; ++i)
-    ok = cudaEventCreateWithFlags(&c->gz2_ready[i], cudaEventDisableTiming) == cudaSuccess &&
-         cudaEventCreateWithFlags(&c->gz1_ready[i], cudaEventDisableTiming) == cudaSuccess &&
-         cudaEventCreateWithFlags(&c->w2_done[i], cudaEventDisableTiming) == cudaSuccess &&
-         cudaEventCreateWithFlags(&c->w1_done[i], cudaEventDisableTiming) == cudaSuccess;
+  for (int k = 0; k < 2 && ok; ++k)
+    for (int i = 0; i < 2 && ok; ++i)
+      ok = cudaEventCreateWithFlags(&c->ready[k][i], cudaEventDisableTiming) == cudaSuccess &&
+           cudaEventCreateWithFlags(&c->done[k][i], cudaEventDisableTiming) == cudaSuccess;
   ok = ok && cudaEventCreateWithFlags(&c->join, cudaEventDisableTiming) == cudaSuccess;
   if (!ok) cudaGetLastError();
   c->ok = ok;
   return ok ? c : nullptr;
 }
 
-// PGNN_EMBED_GEMM=0: embedding-table gradient through the vector-atomics kernel instead of the one-hot GEMM (development switch)
-inline bool embed_gemm_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("PGNN_EMBED_GEMM");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
+// the main stream waits for everything enqueued on the side stream so far
+int join_side(const SideCtx* sc, cudaStream_t st) {
+  PGNN_CUDA(cudaEventRecord(sc->join, sc->side));
+  PGNN_CUDA(cudaStreamWaitEvent(st, sc->join, 0));
+  return PGNN_OK;
 }
 
-#define TRY(call)                 \
-  do {                            \
-    int rc__ = (call);            \
-    if (rc__ != PGNN_OK) return rc__; \
-  } while (0)
+// Graph preparation, the per-node bond summary S (not for GAT, whose kernels read the bond codes per edge), the atom embedding
+// and, for the tensor-path backward, the one-hot atom-code rows.
+int forward_prologue(int type, const Front& f, const void* const* params, const int64_t* x, const int64_t* edge_index,
+                     const int64_t* edge_attr, int64_t N, int64_t E, int64_t D, int training, int precision, void* scratch,
+                     int64_t scratch_bytes, void* stream) {
+  TRY(pgnn_graph_prep(edge_index, E, N, f.rowptr_t, f.nbr_t, f.eid_t, f.rowptr_s, f.nbr_s, f.eid_s, scratch, scratch_bytes, stream));
+  if (type == PGNN_CONV_GCN) TRY(pgnn_gcn_dinv(f.rowptr_t, N, f.dinv, stream));
+  if (type != PGNN_CONV_GAT) TRY(pgnn_chem_edge_summary(edge_attr, f.rowptr_t, f.nbr_t, f.eid_t, N, agg_mode(type), f.dinv, f.S, stream));
+  TRY(pgnn_chem_embed_fwd(x, (const float*)params[P_XEMB1], kAtomRows, (const float*)params[P_XEMB2], kChiralRows, N, D, f.h0, D, stream));
+  if (training && precision == 1) TRY(pgnn_internal_chem_onehot(x, N, kAtomRows, kChiralRows, f.onehot, kOneHotLd, as_stream(stream)));
+  return PGNN_OK;
+}
+
+// Backward tail of every type: the side stream's last wgrad (and its use of the split-K workspace) joins the main stream, then
+// the embedding tables: [120 + 3, D] = onehot^T . gh as a split-K weight-gradient GEMM (the two tables are adjacent in the flat
+// layout); the vector-atomics kernel is the FFMA-precision path and the fallback.
+int embed_backward(const SideCtx* sc, const Front& f, const float* gh, const int64_t* x, int64_t N, int64_t D, int precision,
+                   float* grads, const int64_t* off, float* wpart, int64_t wpart_floats, cudaStream_t st) {
+  if (sc) TRY(join_side(sc, st));
+  int rc = PGNN_EUNSUPPORTED;
+  if (precision == 1)
+    rc = pgnn_tc_linear_bwd_w_ws(f.onehot, kOneHotLd, gh, D, N, kAtomRows + kChiralRows, D, grads + off[P_XEMB1], nullptr, wpart,
+                                 wpart_floats, st);
+  if (rc == PGNN_EUNSUPPORTED)
+    rc = pgnn_chem_embed_bwd(x, gh, D, N, D, grads + off[P_XEMB1], kAtomRows, grads + off[P_XEMB2], kChiralRows, st);
+  return rc;
+}
 
 }  // namespace
 
 extern "C" {
 
-int64_t pgnn_chem_gin_num_params(int64_t L) { return L < 1 ? PGNN_EINVAL : 2 + L_COUNT * L; }
+// ------------------------------------------------------------------------------------------------------------------------------
+// GIN
+// ------------------------------------------------------------------------------------------------------------------------------
+int64_t pgnn_chem_gin_num_params(int64_t L) { return L < 1 ? PGNN_EINVAL : grad_layout(kGin, L, 0, nullptr); }
 
 int pgnn_chem_gin_grad_offsets(int64_t L, int64_t D, int64_t* offsets /*host [num_params + 1]*/) {
   PGNN_CHECK_ARG(L >= 1 && D > 0 && offsets);
-  int64_t o = 0, i = 0;
-  offsets[i++] = o; o += 120 * D;  // x_embedding1.weight
-  offsets[i++] = o; o += 3 * D;    // x_embedding2.weight
-  for (int64_t l = 0; l < L; ++l) {
-    offsets[i++] = o; o += 2 * D * D;  // mlp.0.weight [2D, D]
-    offsets[i++] = o; o += 2 * D;      // mlp.0.bias
-    offsets[i++] = o; o += 2 * D * D;  // mlp.2.weight [D, 2D]
-    offsets[i++] = o; o += D;          // mlp.2.bias
-    offsets[i++] = o; o += 6 * D;      // edge_embedding1.weight
-    offsets[i++] = o; o += 3 * D;      // edge_embedding2.weight
-    offsets[i++] = o; o += D;          // batch_norms.l.weight
-    offsets[i++] = o; o += D;          // batch_norms.l.bias
-  }
-  offsets[i] = o;
+  grad_layout(kGin, L, D, offsets);
   return PGNN_OK;
 }
 
 int64_t pgnn_chem_gin_workspace_bytes(int64_t N, int64_t E, int64_t L, int64_t D) {
   if (N < 0 || E < 0 || L < 1 || D <= 0) return PGNN_EINVAL;
-  return carve(nullptr, N, E, L, D).total;
+  return carve_gin(nullptr, N, E, L, D).total;
 }
 
 // Development / test aid: byte offsets inside the workspace of the saved activations a test needs to reconstruct the
@@ -208,8 +334,8 @@ int64_t pgnn_chem_gin_workspace_bytes(int64_t N, int64_t E, int64_t L, int64_t D
 // layer outputs, [L][N][D]), out[2] = BatchNorm batch mean [L][D], out[3] = invstd [L][D].
 int pgnn_chem_gin_debug_layout(int64_t N, int64_t E, int64_t L, int64_t D, int64_t* out4) {
   PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && out4);
-  char* base = reinterpret_cast<char*>(0x1000);  // carve() only does pointer arithmetic
-  Ws w = carve(base, N, E, L, D);
+  char* base = reinterpret_cast<char*>(0x1000);  // carve_gin() only does pointer arithmetic
+  GinWs w = carve_gin(base, N, E, L, D);
   out4[0] = reinterpret_cast<char*>(w.z1) - base;
   out4[1] = reinterpret_cast<char*>(w.z2) - base;
   out4[2] = reinterpret_cast<char*>(w.mean) - base;
@@ -225,12 +351,8 @@ int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mea
   PGNN_CHECK_ARG(N == 0 || (x && node_rep));
   if (workspace_bytes < pgnn_chem_gin_workspace_bytes(N, E, L, D)) return PGNN_EWORKSPACE;
   if (N == 0) return PGNN_OK;
-  if (training && N < 1) return PGNN_EINVAL;
-  Ws w = carve(workspace, N, E, L, D);
-  TRY(pgnn_graph_prep(edge_index, E, N, w.rowptr_t, w.nbr_t, w.eid_t, w.rowptr_s, w.nbr_s, w.eid_s, w.scratch, w.scratch_bytes, stream));
-  TRY(pgnn_chem_edge_summary(edge_attr, w.rowptr_t, w.nbr_t, w.eid_t, N, PGNN_AGG_SUM, nullptr, w.S, stream));
-  TRY(pgnn_chem_embed_fwd(x, (const float*)params[P_XEMB1], kAtomRows, (const float*)params[P_XEMB2], kChiralRows, N, D, w.h0, D, stream));
-  if (training && precision == 1) TRY(pgnn_internal_chem_onehot(x, N, kAtomRows, kChiralRows, w.onehot, kOneHotLd, as_stream(stream)));
+  GinWs w = carve_gin(workspace, N, E, L, D);
+  TRY(forward_prologue(kGin, w, params, x, edge_index, edge_attr, N, E, D, training, precision, w.scratch, w.scratch_bytes, stream));
   const float* h = w.h0;            // input rows of the current layer (pre-affine)
   const float *in_scale = nullptr, *in_shift = nullptr;
   PgnnBnFold fold;                  // pending BatchNorm finalisation of the previous layer (folded into this layer's gather)
@@ -304,14 +426,14 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
   if (workspace_bytes < pgnn_chem_gin_workspace_bytes(N, E, L, D)) return PGNN_EWORKSPACE;
   int64_t off[2 + L_COUNT * 64 + 1];
   PGNN_CHECK_ARG(L <= 64);
-  pgnn_chem_gin_grad_offsets(L, D, off);
+  grad_layout(kGin, L, D, off);
   cudaStream_t st = as_stream(stream);
   if (N == 0) {
     PGNN_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * off[2 + L_COUNT * L], st));
     return PGNN_OK;
   }
   PGNN_CHECK_ARG(g_node_rep && x);
-  Ws w = carve(workspace, N, E, L, D);
+  GinWs w = carve_gin(workspace, N, E, L, D);
   // transposed copies of the 2L MLP weights: with them every dgrad has both operands reduction-contiguous, and the GEMM
   // stores its operand tiles without a transpose
   bool have_wT = false;
@@ -343,7 +465,7 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
     float* gz2 = w.gz2 + (sc ? par * N * D : 0);
     float* gz1 = w.gz1 + (sc ? par * N * 2 * D : 0);
     // BatchNorm (+ReLU mask recomputed from z2) backward; the same pass leaves colsum(gz2) = gradient of mlp.2.bias
-    if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->w2_done[par], 0));  // layer l+2's wgrad2 has finished reading this copy
+    if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad2 has finished reading this copy
     TRY(pgnn_internal_bn_bwd_colsum(gy, ldgy, z2, D, N, D, (const float*)p[L_GAMMA], (const float*)p[L_BETA], w.mean + l * D,
                                     w.invstd + l * D, !last, gz2, D, grads + o[L_GAMMA], grads + o[L_BETA], grads + o[L_B2],
                                     w.scratch, st));
@@ -352,14 +474,14 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
     bool fused = false;
     if (precision == 1) {
       if (sc) {
-        PGNN_CUDA(cudaEventRecord(sc->gz2_ready[par], st));
-        PGNN_CUDA(cudaStreamWaitEvent(wst, sc->gz2_ready[par], 0));
+        PGNN_CUDA(cudaEventRecord(sc->ready[0][par], st));
+        PGNN_CUDA(cudaStreamWaitEvent(wst, sc->ready[0][par], 0));
       }
       int rc = pgnn_tc_linear_bwd_w_ws(gz2, D, z1, 2 * D, N, D, 2 * D, grads + o[L_W2], nullptr, w.wpart, w.wpart_floats, wst);
       if (rc == PGNN_OK) {
         if (sc) {
-          PGNN_CUDA(cudaEventRecord(sc->w2_done[par], wst));
-          PGNN_CUDA(cudaStreamWaitEvent(st, sc->w1_done[par], 0));  // layer l+2's wgrad1 has finished reading gz1[par]
+          PGNN_CUDA(cudaEventRecord(sc->done[0][par], wst));
+          PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[1][par], 0));  // layer l+2's wgrad1 has finished reading gz1[par]
         }
         PGNN_CUDA(cudaMemsetAsync(grads + o[L_B1], 0, sizeof(float) * 2 * D, st));
         PgnnGemmHooks h1;
@@ -370,12 +492,12 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
           rc = pgnn_tc_linear_bwd_x(gz2, D, (const float*)p[L_W2], N, D, 2 * D, z1, 2 * D, gz1, 2 * D, st, &h1);
         if (rc != PGNN_OK) return rc;
         if (sc) {
-          PGNN_CUDA(cudaEventRecord(sc->gz1_ready[par], st));
-          PGNN_CUDA(cudaStreamWaitEvent(wst, sc->gz1_ready[par], 0));
+          PGNN_CUDA(cudaEventRecord(sc->ready[1][par], st));
+          PGNN_CUDA(cudaStreamWaitEvent(wst, sc->ready[1][par], 0));
         }
         rc = pgnn_tc_linear_bwd_w_ws(gz1, 2 * D, aggr, D, N, 2 * D, D, grads + o[L_W1], nullptr, w.wpart, w.wpart_floats, wst);
         if (rc != PGNN_OK) return rc;
-        if (sc) PGNN_CUDA(cudaEventRecord(sc->w1_done[par], wst));
+        if (sc) PGNN_CUDA(cudaEventRecord(sc->done[1][par], wst));
         PGNN_CUDA(cudaMemsetAsync(grads + o[L_ET1], 0, sizeof(float) * 9 * D, st));  // the two tables are adjacent in the layout
         PgnnGemmHooks h2;
         h2.S = w.S; h2.Q = 9; h2.gT = grads + o[L_ET1]; h2.gT2 = grads + o[L_ET2]; h2.q_split = 6; h2.ldt = D;
@@ -390,10 +512,7 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
       }
     }
     if (!fused) {
-      if (sc) {  // an unsupported shape on the tensor path: everything on the caller's stream from here on
-        PGNN_CUDA(cudaEventRecord(sc->join, wst));
-        PGNN_CUDA(cudaStreamWaitEvent(st, sc->join, 0));
-      }
+      if (sc) TRY(join_side(sc, st));  // an unsupported shape on the tensor path: everything on the caller's stream from here on
       TRY(pgnn_linear_bwd_w(gz2, D, z1, 2 * D, N, D, 2 * D, grads + o[L_W2], nullptr, precision, stream));
       TRY(pgnn_linear_bwd_x(gz2, D, (const float*)p[L_W2], N, D, 2 * D, z1, 2 * D, gz1, 2 * D, precision, stream));
       TRY(pgnn_linear_bwd_w(gz1, 2 * D, aggr, D, N, 2 * D, D, grads + o[L_W1], grads + o[L_B1], precision, stream));
@@ -407,19 +526,152 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
     gy = w.gh;
     ldgy = D;
   }
-  if (sc) {  // the side stream's last wgrad (and its use of the split-K workspace) before the embedding GEMM and before returning
-    PGNN_CUDA(cudaEventRecord(sc->join, wst));
-    PGNN_CUDA(cudaStreamWaitEvent(st, sc->join, 0));
+  return embed_backward(sc, w, w.gh, x, N, D, precision, grads, off, w.wpart, w.wpart_floats, st);
+}
+
+// ------------------------------------------------------------------------------------------------------------------------------
+// GCN / GraphSAGE / GAT
+// ------------------------------------------------------------------------------------------------------------------------------
+int64_t pgnn_chem_conv_num_params(int conv_type, int64_t L) {
+  if (!valid_conv(conv_type) || L < 1) return PGNN_EINVAL;
+  return grad_layout(conv_type, L, 0, nullptr);
+}
+
+int pgnn_chem_conv_grad_offsets(int conv_type, int64_t L, int64_t D, int64_t* offsets) {
+  PGNN_CHECK_ARG(valid_conv(conv_type) && L >= 1 && D > 0 && offsets);
+  grad_layout(conv_type, L, D, offsets);
+  return PGNN_OK;
+}
+
+int64_t pgnn_chem_conv_workspace_bytes(int conv_type, int64_t N, int64_t E, int64_t L, int64_t D) {
+  if (!valid_conv(conv_type) || N < 0 || E < 0 || L < 1 || D <= 0) return PGNN_EINVAL;
+  return carve_conv(nullptr, conv_type, N, E, L, D).total;
+}
+
+int pgnn_chem_conv_forward(int conv_type, const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
+                           void* const* bn_num_batches_tracked, const int64_t* x, const int64_t* edge_index, const int64_t* edge_attr,
+                           int64_t N, int64_t E, int64_t L, int64_t D, int training, float momentum, float eps, int precision,
+                           float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes, void* stream) {
+  PGNN_CHECK_ARG(valid_conv(conv_type) && N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && bn_running_mean && bn_running_var &&
+                 workspace);
+  PGNN_CHECK_ARG(N == 0 || (x && node_rep));
+  PGNN_CHECK_ARG(E == 0 || (edge_index && edge_attr));
+  if (workspace_bytes < pgnn_chem_conv_workspace_bytes(conv_type, N, E, L, D)) return PGNN_EWORKSPACE;
+  if (N == 0) return PGNN_OK;
+  cudaStream_t st = as_stream(stream);
+  const bool gat = conv_type == PGNN_CONV_GAT;
+  const int64_t HD = gat ? kHeads * D : D;
+  const int PL = layer_params(conv_type);
+  ConvWs w = carve_conv(workspace, conv_type, N, E, L, D);
+  TRY(forward_prologue(conv_type, w, params, x, edge_index, edge_attr, N, E, D, training, precision, w.scratch, w.scratch_bytes, stream));
+  const float* h = w.h0;
+  for (int64_t l = 0; l < L; ++l) {
+    const void* const* p = params + P_LAYER0 + l * PL;
+    const bool last = l == L - 1;
+    float* xl = w.xl + l * N * HD;
+    float* z = w.z + l * N * D;
+    float* hout = last ? node_rep : w.hout + l * N * D;
+    const int64_t ldh = last ? ld_out : D;
+    TRY(pgnn_linear_fwd(h, D, (const float*)p[gat ? A_W : G_W], (const float*)p[gat ? A_B : G_B], N, HD, D, 0, xl, HD, precision, stream));
+    if (gat) {
+      float* T = w.T + l * 9 * HD;  // the kernels index one [9, H*D] table: rows 0..5 bond type, 6..8 bond direction
+      PGNN_CUDA(cudaMemcpyAsync(T, p[A_ET1], sizeof(float) * 6 * HD, cudaMemcpyDeviceToDevice, st));
+      PGNN_CUDA(cudaMemcpyAsync(T + 6 * HD, p[A_ET2], sizeof(float) * 3 * HD, cudaMemcpyDeviceToDevice, st));
+      TRY(pgnn_gat_fwd(xl, N, kHeads, D, (const float*)p[A_ATT], T, 0, edge_attr, w.rowptr_t, w.nbr_t, w.eid_t, E, (const float*)p[A_BIAS], kSlope,
+                       w.alpha + l * (E + N) * kHeads, w.pq + l * N * kHeads * 2, z, D, stream));
+    } else if (conv_type == PGNN_CONV_GCN) {
+      TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_GCN, w.dinv, w.S, 9, (const float*)p[G_ET1],
+                                      (const float*)p[G_ET2], 6, 0, z, D, st, nullptr));
+    } else {
+      // mean aggregation into the backward scratch `gz` (only its normalised rows and their norms are needed later)
+      TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_MEAN, nullptr, w.S, 9, (const float*)p[G_ET1],
+                                      (const float*)p[G_ET2], 6, 0, w.gz, D, st, nullptr));
+      TRY(pgnn_l2norm_fwd(w.gz, D, N, D, z, D, w.nrm + l * N, stream));
+    }
+    const float* gamma = (const float*)p[gat ? A_GAMMA : G_GAMMA];
+    const float* beta = (const float*)p[gat ? A_BETA : G_BETA];
+    if (training) {
+      TRY(pgnn_bn_fwd_train(z, D, N, D, gamma, beta, (float*)bn_running_mean[l], (float*)bn_running_var[l],
+                            bn_num_batches_tracked ? (int64_t*)bn_num_batches_tracked[l] : nullptr, momentum, eps, !last, hout, ldh, w.mean + l * D,
+                            w.invstd + l * D, nullptr, nullptr, w.scratch, w.scratch_bytes, stream));
+    } else {
+      TRY(pgnn_bn_fwd_eval(z, D, N, D, gamma, beta, (const float*)bn_running_mean[l], (const float*)bn_running_var[l], eps, !last, hout, ldh, stream));
+    }
+    h = hout;
   }
-  // embedding tables: [120 + 3, D] = onehot^T . gh as a split-K weight-gradient GEMM (the two tables are adjacent in the flat
-  // layout); the vector-atomics kernel remains the fallback (FFMA precision)
-  int rc_e = PGNN_EUNSUPPORTED;
-  if (precision == 1 && embed_gemm_enabled() && off[P_XEMB2] == off[P_XEMB1] + (int64_t)kAtomRows * D)
-    rc_e = pgnn_tc_linear_bwd_w_ws(w.onehot, kOneHotLd, w.gh, D, N, kAtomRows + kChiralRows, D, grads + off[P_XEMB1], nullptr, w.wpart,
-                                   w.wpart_floats, st);
-  if (rc_e == PGNN_EUNSUPPORTED)
-    rc_e = pgnn_chem_embed_bwd(x, w.gh, D, N, D, grads + off[P_XEMB1], kAtomRows, grads + off[P_XEMB2], kChiralRows, stream);
-  return rc_e;
+  return PGNN_OK;
+}
+
+int pgnn_chem_conv_backward(int conv_type, const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x,
+                            const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, int precision, float* grads,
+                            void* workspace, int64_t workspace_bytes, void* stream) {
+  PGNN_CHECK_ARG(valid_conv(conv_type) && N >= 0 && E >= 0 && L >= 1 && L <= 64 && D > 0 && D % 4 == 0 && params && grads && workspace);
+  if (workspace_bytes < pgnn_chem_conv_workspace_bytes(conv_type, N, E, L, D)) return PGNN_EWORKSPACE;
+  int64_t off[2 + A_COUNT * 64 + 1];
+  grad_layout(conv_type, L, D, off);
+  cudaStream_t st = as_stream(stream);
+  const bool gat = conv_type == PGNN_CONV_GAT;
+  const int64_t HD = gat ? kHeads * D : D;
+  const int PL = layer_params(conv_type);
+  if (N == 0) {
+    PGNN_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * off[2 + PL * L], st));
+    return PGNN_OK;
+  }
+  PGNN_CHECK_ARG(g_node_rep && x && (E == 0 || edge_attr));
+  ConvWs w = carve_conv(workspace, conv_type, N, E, L, D);
+  const float* gy = g_node_rep;
+  int64_t ldgy = ldg;
+  SideCtx* sc = precision == 1 ? side_ctx(st) : nullptr;
+  cudaStream_t wst = sc ? sc->side : st;
+  for (int64_t l = L - 1; l >= 0; --l) {
+    const void* const* p = params + P_LAYER0 + l * PL;
+    const int64_t* o = off + P_LAYER0 + l * PL;
+    const bool last = l == L - 1;
+    const int par = (int)(l & 1);
+    const float* xl = w.xl + l * N * HD;
+    const float* z = w.z + l * N * D;
+    const float* hin = l == 0 ? w.h0 : w.hout + (l - 1) * N * D;
+    float* gxl = w.gxl + (sc ? par * N * HD : 0);
+    const float* gamma = (const float*)p[gat ? A_GAMMA : G_GAMMA];
+    const float* beta = (const float*)p[gat ? A_BETA : G_BETA];
+    TRY(pgnn_bn_bwd(gy, ldgy, z, D, N, D, gamma, beta, w.mean + l * D, w.invstd + l * D, !last, w.gz, D, grads + o[gat ? A_GAMMA : G_GAMMA],
+                    grads + o[gat ? A_BETA : G_BETA], w.scratch, w.scratch_bytes, stream));
+    if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad has finished reading this copy of gxl
+    if (gat) {
+      // gT [9, HD] lands on the two adjacent bond-table gradients
+      TRY(pgnn_gat_bwd(w.gz, D, xl, N, kHeads, D, (const float*)p[A_ATT], w.T + l * 9 * HD, 0, edge_attr, w.rowptr_t, w.nbr_t, w.eid_t, w.rowptr_s,
+                       w.nbr_s, w.eid_s, E, kSlope, w.alpha + l * (E + N) * kHeads, w.pq + l * N * kHeads * 2, gxl, grads + o[A_ATT],
+                       grads + o[A_ET1], grads + o[A_BIAS], w.scratch, w.scratch_bytes, stream));
+    } else {
+      const float* ga = w.gz;
+      if (conv_type == PGNN_CONV_SAGE) {
+        TRY(pgnn_l2norm_bwd(w.gz, D, z, D, w.nrm + l * N, N, D, w.ga, D, stream));
+        ga = w.ga;
+      }
+      PGNN_CUDA(cudaMemsetAsync(grads + o[G_ET1], 0, sizeof(float) * 9 * D, st));
+      TRY(pgnn_internal_edge_table_bwd2(w.S, 9, ga, D, 0, N, (int)D, grads + o[G_ET1], D, grads + o[G_ET2], 6, st));
+      TRY(pgnn_aggregate_bwd(ga, D, N, D, w.rowptr_s, w.nbr_s, agg_mode(conv_type), w.dinv, w.rowptr_t, gxl, D, stream));
+    }
+    // Linear backward: weight + bias gradients (side stream), then the input gradient
+    if (sc) {
+      PGNN_CUDA(cudaEventRecord(sc->ready[0][par], st));
+      PGNN_CUDA(cudaStreamWaitEvent(wst, sc->ready[0][par], 0));
+    }
+    int rc = PGNN_EUNSUPPORTED;
+    if (precision == 1)
+      rc = pgnn_tc_linear_bwd_w_ws(gxl, HD, hin, D, N, HD, D, grads + o[gat ? A_W : G_W], grads + o[gat ? A_B : G_B], w.wpart, w.wpart_floats, wst);
+    if (rc == PGNN_EUNSUPPORTED) {
+      if (sc) TRY(join_side(sc, st));
+      rc = pgnn_linear_bwd_w(gxl, HD, hin, D, N, HD, D, grads + o[gat ? A_W : G_W], grads + o[gat ? A_B : G_B], precision, stream);
+    } else if (sc) {
+      PGNN_CUDA(cudaEventRecord(sc->done[0][par], wst));
+    }
+    if (rc != PGNN_OK) return rc;
+    TRY(pgnn_linear_bwd_x(gxl, HD, (const float*)p[gat ? A_W : G_W], N, HD, D, nullptr, 0, w.gh, D, precision, stream));
+    gy = w.gh;
+    ldgy = D;
+  }
+  return embed_backward(sc, w, w.gh, x, N, D, precision, grads, off, w.wpart, w.wpart_floats, st);
 }
 
 }  // extern "C"

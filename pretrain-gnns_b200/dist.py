@@ -286,7 +286,7 @@ class GradAllReducer:
 
 def encoder_flat_source(gnn):
     """flat_sources entry for a chem GNN running the fused path: (last flat gradient buffer, its parameters).
-    `bind(buffer)` makes the encoder's backward write its gradients into `buffer` (see ChemGinPlan.grad_buffer)."""
+    `bind(buffer)` makes the encoder's backward write its gradients into `buffer` (see ChemEncoderPlan.grad_buffer)."""
     def src():
         plan = gnn._fused_plan()
         if plan is None:

@@ -644,36 +644,57 @@ def gat(xl, att, T, edge_attr, graph, bias, heads=2, slope=0.2, is_bio=False):
 
 
 # ------------------------------------------------------------------------------------------------
-# whole-encoder fast path: chem GIN (pgnn_chem_gin_forward / pgnn_chem_gin_backward)
+# whole-encoder fast path: chem GIN (pgnn_chem_gin_*) and GCN / GraphSAGE / GAT (pgnn_chem_conv_*)
 # ------------------------------------------------------------------------------------------------
 import ctypes as _ct
 
+CONV_TYPE = {"gcn": 1, "graphsage": 2, "gat": 3}
 
-class ChemGinPlan:
-    """Per-module bookkeeping for the fused chem GIN encoder: parameter order, gradient layout, pointer tables."""
 
-    def __init__(self, gnn):
+def _layer_params(gnn_type, conv):
+    """One conv's parameters in the order of include/pgnn_b200.h (also the flat gradient order)."""
+    if gnn_type == "gin":
+        ps = [conv.mlp[0].weight, conv.mlp[0].bias, conv.mlp[2].weight, conv.mlp[2].bias]
+    elif gnn_type == "gat":
+        ps = [conv.weight_linear.weight, conv.weight_linear.bias, conv.att, conv.bias]
+    else:
+        ps = [conv.linear.weight, conv.linear.bias]
+    return ps + [conv.edge_embedding1.weight, conv.edge_embedding2.weight]
+
+
+class ChemEncoderPlan:
+    """Per-module bookkeeping for the whole-encoder chem GNN: parameter order, gradient layout, pointer tables, and the C calls.
+    GIN runs on pgnn_chem_gin_*, gcn | graphsage | gat on pgnn_chem_conv_*; the plan's methods are the only code that tells them
+    apart."""
+
+    def __init__(self, gnn, gnn_type):
+        self.gnn_type = gnn_type
+        self.conv = 0 if gnn_type == "gin" else CONV_TYPE[gnn_type]
         self.L = len(gnn.gnns)
         self.D = gnn.x_embedding1.weight.shape[1]
         ps = [gnn.x_embedding1.weight, gnn.x_embedding2.weight]
         for conv, bn in zip(gnn.gnns, gnn.batch_norms):
-            ps += [conv.mlp[0].weight, conv.mlp[0].bias, conv.mlp[2].weight, conv.mlp[2].bias,
-                   conv.edge_embedding1.weight, conv.edge_embedding2.weight, bn.weight, bn.bias]
+            ps += _layer_params(gnn_type, conv) + [bn.weight, bn.bias]
         self.params = ps
         n = len(ps)
-        assert n == lib.pgnn_chem_gin_num_params(self.L)
         off = (_ct.c_int64 * (n + 1))()
-        check(lib.pgnn_chem_gin_grad_offsets(self.L, self.D, off), "chem_gin_grad_offsets")
+        if self.conv:
+            assert n == lib.pgnn_chem_conv_num_params(self.conv, self.L)
+            check(lib.pgnn_chem_conv_grad_offsets(self.conv, self.L, self.D, off), "chem_conv_grad_offsets")
+        else:
+            assert n == lib.pgnn_chem_gin_num_params(self.L)
+            check(lib.pgnn_chem_gin_grad_offsets(self.L, self.D, off), "chem_gin_grad_offsets")
         self.offsets = list(off)
         self.sizes = [self.offsets[i + 1] - self.offsets[i] for i in range(n)]
         self.shapes = [tuple(p.shape) for p in ps]
         for p, s in zip(ps, self.sizes):
             if p.numel() != s:
-                raise PgnnError("parameter shape does not match the chem GIN layout (emb_dim / vocabulary sizes)")
+                raise PgnnError("parameter shape does not match the chem %s layout (emb_dim / heads / vocabulary sizes)" % gnn_type)
         self.total = self.offsets[-1]
         self.PtrArr = _ct.c_void_p * n
         self.BnArr = _ct.c_void_p * self.L
         self.bns = list(gnn.batch_norms)
+        self._ws_alloc = 0          # workspace bytes requested from the allocator so far (see workspace_bytes)
         self.last_flat_grad = None  # the flat gradient buffer of the most recent backward (all-reduce target)
         # optional caller-owned destination ([total] fp32, e.g. a slice of NVLink-symmetric memory): used instead of a fresh
         # buffer whenever no parameter still holds a gradient (autograd would otherwise add a view of the buffer to itself)
@@ -683,26 +704,46 @@ class ChemGinPlan:
         # would overwrite the buffer whose views the engine still holds as the first node's gradients.  (A forward whose
         # graph is dropped without a backward leaves the count raised: the fresh-buffer path is then taken, which is safe.)
         self.live_forwards = 0
-        self.keep_workspace = False   # tests: keep the last training forward's workspace (relu_masks)
+        self.direct_grads = True    # False: every gradient goes back through autograd (see _deliver_flat_grads)
+        self._own_flat = None       # the plan's own flat gradient buffer when no grad_buffer is bound
+        self._views = None          # (data_ptr, per-parameter views) of the last fast-path flat buffer
+        self.keep_workspace = False  # GIN tests: keep the last training forward's workspace (chem_gin_relu_masks)
         self.last_ws = None
 
+    def workspace_bytes(self, N, E):
+        """Workspace size actually requested from the allocator: the largest need seen so far plus headroom, rounded to 16 MiB.
+        Batches differ by a few percent in N and E; asking for exactly the need makes every new maximum a cudaMalloc
+        (milliseconds, and a device synchronisation) in the middle of training, whereas one size per plan is served from the
+        caching allocator's free list."""
+        if self.conv:
+            need = lib.pgnn_chem_conv_workspace_bytes(self.conv, N, E, self.L, self.D)
+        else:
+            need = lib.pgnn_chem_gin_workspace_bytes(N, E, self.L, self.D)
+        if need < 0:
+            return need
+        if need > self._ws_alloc:
+            self._ws_alloc = ((need + need // 16) + (16 << 20) - 1) // (16 << 20) * (16 << 20)
+        return self._ws_alloc
 
-def _grow_only(plan, need):
-    """Workspace size actually requested from the allocator: the largest need seen so far plus headroom, rounded to 16 MiB.  Batches
-    differ by a few percent in N and E; asking for exactly `need` makes every new maximum a cudaMalloc (milliseconds, and a device
-    synchronisation) in the middle of training, whereas one size per plan is served from the caching allocator's free list."""
-    if need < 0:
-        return need
-    cur = getattr(plan, "_ws_alloc", 0)
-    if need > cur:
-        cur = ((need + need // 16) + (16 << 20) - 1) // (16 << 20) * (16 << 20)
-        plan._ws_alloc = cur
-    return cur
+    def forward(self, ptrs, rm, rv, nbt, x, ei, ea, N, E, training, momentum, eps, out, ws, wsb):
+        args = (ptrs, rm, rv, nbt, _p(x), _p(ei), _p(ea), N, E, self.L, self.D, int(training), float(momentum), float(eps),
+                _precision, _p(out), self.D, _p(ws), wsb, _st())
+        if self.conv:
+            check(lib.pgnn_chem_conv_forward(self.conv, *args), "chem_conv_forward")
+        else:
+            check(lib.pgnn_chem_gin_forward(*args), "chem_gin_forward")
 
+    def backward(self, ptrs, g, x, ea, N, E, flat, ws, wsb):
+        if self.conv:
+            check(lib.pgnn_chem_conv_backward(self.conv, ptrs, _p(g), g.stride(0), _p(x), _p(ea), N, E, self.L, self.D, _precision,
+                                              _p(flat), _p(ws), wsb, _st()), "chem_conv_backward")
+        else:
+            check(lib.pgnn_chem_gin_backward(ptrs, _p(g), g.stride(0), _p(x), N, E, self.L, self.D, _precision, _p(flat), _p(ws),
+                                             wsb, _st()), "chem_gin_backward")
 
 
 def _deliver_flat_grads(plan, ctx, run):
-    """Shared tail of the whole-encoder backwards: pick the flat gradient buffer, run the C backward into it (`run(flat)`), and hand
+    """Tail of the whole-encoder backward: pick the flat gradient buffer, run the C backward into it (`run(flat)`), and hand
     the per-parameter views to autograd.
 
     Fast path (the normal training step: one live forward, no parameter holds a gradient yet, every parameter is a leaf that
@@ -716,13 +757,13 @@ def _deliver_flat_grads(plan, ctx, run):
     plan.live_forwards = max(plan.live_forwards - 1, 0)
     needs = ctx.needs_input_grad[5:]
     clean = sole and all(p.grad is None for p in params)
-    if clean and getattr(plan, "direct_grads", True) and all(needs) and all(p.is_leaf for p in params):
+    if clean and plan.direct_grads and all(needs) and all(p.is_leaf for p in params):
         flat = plan.grad_buffer
         if flat is None:
-            flat = getattr(plan, "_own_flat", None)
+            flat = plan._own_flat
             if flat is None or flat.device != ctx.x.device:
                 flat = plan._own_flat = torch.empty(plan.total, dtype=torch.float32, device=ctx.x.device)
-        cache = getattr(plan, "_views", None)
+        cache = plan._views
         if cache is None or cache[0] != flat.data_ptr():
             cache = plan._views = (flat.data_ptr(), [v.view(s) for v, s in zip(flat.split(plan.sizes), plan.shapes)])
         run(flat)
@@ -740,20 +781,17 @@ def _deliver_flat_grads(plan, ctx, run):
     return (None, None, None, None, None) + tuple(gr if need else None for gr, need in zip(grads, needs))
 
 
-
 def _release_ctx(ctx):
     """Drop the encoder node's references to its ~200 MB workspace and inputs once the backward has been enqueued.  They are plain
     ctx attributes (not save_for_backward tensors), so autograd does not free them with the graph's buffers: as long as the caller
     keeps the loss tensor (e.g. to log it after the NEXT step has started), loss.grad_fn keeps this node and the node kept the
     workspace, the next forward then needed a second one, and that cudaMalloc (40 ms, device-synchronising) was the stall seen at
-    step 1 of every end-to-end loop.  A second backward through the same graph is not supported by these ops anyway."""
-    ctx.ws = ctx.keep = ctx.ptrs = ctx.x = None
-    if hasattr(ctx, "ea"):
-        ctx.ea = None
+    step 1 of every end-to-end loop.  A second backward through the same graph is not supported by this op anyway."""
+    ctx.ws = ctx.keep = ctx.ptrs = ctx.x = ctx.ea = None
     ctx.released = True
 
 
-class _ChemGinEncoder(Function):
+class _ChemEncoder(Function):
     @staticmethod
     def forward(ctx, plan, x, edge_index, edge_attr, training, *params):
         _dev(x, edge_index, edge_attr, *params)
@@ -762,7 +800,7 @@ class _ChemGinEncoder(Function):
         if edge_index.dtype != torch.int64 or edge_index.dim() != 2 or edge_index.shape[0] != 2:
             raise PgnnError("edge_index must be int64 [2, E]")
         x, ei, ea = x.contiguous(), edge_index.contiguous(), edge_attr.contiguous()
-        N, E, L, D = x.shape[0], ei.shape[1], plan.L, plan.D
+        N, E, D = x.shape[0], ei.shape[1], plan.D
         if ea.dtype != torch.int64 or tuple(ea.shape) != (E, 2):
             raise PgnnError("chem edge_attr must be int64 [E, 2]")
         for p in params:
@@ -776,16 +814,15 @@ class _ChemGinEncoder(Function):
         rm = plan.BnArr(*[b.running_mean.data_ptr() for b in bns])
         rv = plan.BnArr(*[b.running_var.data_ptr() for b in bns])
         nbt = plan.BnArr(*[b.num_batches_tracked.data_ptr() for b in bns])
-        wsb = _grow_only(plan, lib.pgnn_chem_gin_workspace_bytes(N, E, L, D))
+        wsb = plan.workspace_bytes(N, E)
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
         out = torch.empty(N, D, dtype=torch.float32, device=dev)
         mom = bns[0].momentum if bns[0].momentum is not None else 0.1
-        check(lib.pgnn_chem_gin_forward(ptrs, rm, rv, nbt, _p(x), _p(ei), _p(ea), N, E, L, D, int(training), float(mom),
-                                        float(bns[0].eps), _precision, _p(out), D, _p(ws), wsb, _st()), "chem_gin_forward")
-        ctx.plan, ctx.ws, ctx.wsb, ctx.ptrs, ctx.x, ctx.dims, ctx.training = plan, ws, wsb, ptrs, x, (N, E, L, D), training
+        plan.forward(ptrs, rm, rv, nbt, x, ei, ea, N, E, training, mom, bns[0].eps, out, ws, wsb)
+        ctx.plan, ctx.ws, ctx.wsb, ctx.ptrs, ctx.x, ctx.ea, ctx.dims, ctx.training = plan, ws, wsb, ptrs, x, ea, (N, E), training
         ctx.keep = params  # the pointer table refers to these storages
         if training and plan.keep_workspace:
-            plan.last_ws = (ws, (N, E, L, D))
+            plan.last_ws = (ws, (N, E, plan.L, D))
         if training and any(ctx.needs_input_grad[5:]):
             plan.live_forwards += 1
         if _VALIDATE:
@@ -800,20 +837,22 @@ class _ChemGinEncoder(Function):
             raise PgnnError("the whole-encoder op released its workspace after its first backward: a second backward through the same "
                             "graph (retain_graph) is not supported; set model.fused = False for that")
         plan = ctx.plan
-        N, E, L, D = ctx.dims
+        N, E = ctx.dims
         g = _f32(g)
-
-        def run(flat):
-            check(lib.pgnn_chem_gin_backward(ctx.ptrs, _p(g), g.stride(0), _p(ctx.x), N, E, L, D, _precision, _p(flat), _p(ctx.ws),
-                                             ctx.wsb, _st()), "chem_gin_backward")
-        out = _deliver_flat_grads(plan, ctx, run)
+        out = _deliver_flat_grads(plan, ctx, lambda flat: plan.backward(ctx.ptrs, g, ctx.x, ctx.ea, N, E, flat, ctx.ws, ctx.wsb))
         _release_ctx(ctx)
         return out
 
 
-def chem_gin_relu_masks(plan: ChemGinPlan, gnn):
+def chem_encoder(plan: ChemEncoderPlan, x, edge_index, edge_attr, training: bool):
+    return _ChemEncoder.apply(plan, x, edge_index, edge_attr, training, *plan.params)
+
+
+def chem_gin_relu_masks(plan: ChemEncoderPlan, gnn):
     """The ReLU decisions of the last training forward of the fused GIN encoder (plan.keep_workspace = True), in the order the
     reference takes them: per layer the MLP's hidden units [N, 2D], then (all but the last layer) the post-BatchNorm units [N, D]."""
+    if plan.gnn_type != "gin":
+        raise PgnnError("chem_gin_relu_masks reads the GIN workspace layout (pgnn_chem_gin_debug_layout)")
     ws, (N, E, L, D) = plan.last_ws
     off = (_ct.c_int64 * 4)()
     check(lib.pgnn_chem_gin_debug_layout(N, E, L, D, off), "chem_gin_debug_layout")
@@ -829,110 +868,6 @@ def chem_gin_relu_masks(plan: ChemGinPlan, gnn):
             xhat = (z2[l] - mean[l]) * invstd[l]
             masks.append(torch.addcmul(bn.bias.detach(), xhat, bn.weight.detach()) > 0)   # the backward's own test: fma(xhat, gamma, beta) > 0
     return masks
-
-
-def chem_gin_encoder(plan: ChemGinPlan, x, edge_index, edge_attr, training: bool):
-    return _ChemGinEncoder.apply(plan, x, edge_index, edge_attr, training, *plan.params)
-
-
-# ------------------------------------------------------------------------------------------------
-# whole-encoder fast path: chem GCN / GraphSAGE / GAT (pgnn_chem_conv_forward / pgnn_chem_conv_backward)
-# ------------------------------------------------------------------------------------------------
-CONV_TYPE = {"gcn": 1, "graphsage": 2, "gat": 3}
-
-
-class ChemConvPlan:
-    """Same bookkeeping as ChemGinPlan for gnn_type = gcn | graphsage | gat (parameter order of include/pgnn_b200.h)."""
-
-    def __init__(self, gnn, gnn_type):
-        self.conv = CONV_TYPE[gnn_type]
-        self.L = len(gnn.gnns)
-        self.D = gnn.x_embedding1.weight.shape[1]
-        ps = [gnn.x_embedding1.weight, gnn.x_embedding2.weight]
-        for conv, bn in zip(gnn.gnns, gnn.batch_norms):
-            if gnn_type == "gat":
-                ps += [conv.weight_linear.weight, conv.weight_linear.bias, conv.att, conv.bias]
-            else:
-                ps += [conv.linear.weight, conv.linear.bias]
-            ps += [conv.edge_embedding1.weight, conv.edge_embedding2.weight, bn.weight, bn.bias]
-        self.params = ps
-        n = len(ps)
-        assert n == lib.pgnn_chem_conv_num_params(self.conv, self.L)
-        off = (_ct.c_int64 * (n + 1))()
-        check(lib.pgnn_chem_conv_grad_offsets(self.conv, self.L, self.D, off), "chem_conv_grad_offsets")
-        self.offsets = list(off)
-        self.sizes = [self.offsets[i + 1] - self.offsets[i] for i in range(n)]
-        self.shapes = [tuple(p.shape) for p in ps]
-        for p, s in zip(ps, self.sizes):
-            if p.numel() != s:
-                raise PgnnError("parameter shape does not match the chem %s layout (emb_dim / heads / vocabulary sizes)" % gnn_type)
-        self.total = self.offsets[-1]
-        self.PtrArr = _ct.c_void_p * n
-        self.BnArr = _ct.c_void_p * self.L
-        self.bns = list(gnn.batch_norms)
-        self.last_flat_grad = None
-        self.grad_buffer = None
-        self.live_forwards = 0
-
-
-class _ChemConvEncoder(Function):
-    @staticmethod
-    def forward(ctx, plan, x, edge_index, edge_attr, training, *params):
-        _dev(x, edge_index, edge_attr, *params)
-        if x.dtype != torch.int64 or x.dim() != 2 or x.shape[1] != 2:
-            raise PgnnError("chem node features must be int64 [N, 2]")
-        if edge_index.dtype != torch.int64 or edge_index.dim() != 2 or edge_index.shape[0] != 2:
-            raise PgnnError("edge_index must be int64 [2, E]")
-        x, ei, ea = x.contiguous(), edge_index.contiguous(), edge_attr.contiguous()
-        N, E, L, D = x.shape[0], ei.shape[1], plan.L, plan.D
-        if ea.dtype != torch.int64 or tuple(ea.shape) != (E, 2):
-            raise PgnnError("chem edge_attr must be int64 [E, 2]")
-        for p in params:
-            if p.dtype != torch.float32 or not p.is_contiguous():
-                raise PgnnError("the fused encoder needs contiguous fp32 parameters")
-        if training and N == 0:
-            raise PgnnError("BatchNorm in training mode needs at least one node")
-        dev = x.device
-        ptrs = plan.PtrArr(*[p.data_ptr() for p in params])
-        bns = plan.bns
-        rm = plan.BnArr(*[b.running_mean.data_ptr() for b in bns])
-        rv = plan.BnArr(*[b.running_var.data_ptr() for b in bns])
-        nbt = plan.BnArr(*[b.num_batches_tracked.data_ptr() for b in bns])
-        wsb = _grow_only(plan, lib.pgnn_chem_conv_workspace_bytes(plan.conv, N, E, L, D))
-        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-        out = torch.empty(N, D, dtype=torch.float32, device=dev)
-        mom = bns[0].momentum if bns[0].momentum is not None else 0.1
-        check(lib.pgnn_chem_conv_forward(plan.conv, ptrs, rm, rv, nbt, _p(x), _p(ei), _p(ea), N, E, L, D, int(training), float(mom),
-                                         float(bns[0].eps), _precision, _p(out), D, _p(ws), wsb, _st()), "chem_conv_forward")
-        ctx.plan, ctx.ws, ctx.wsb, ctx.ptrs, ctx.x, ctx.ea, ctx.dims, ctx.training = plan, ws, wsb, ptrs, x, ea, (N, E, L, D), training
-        ctx.keep = params
-        if training and any(ctx.needs_input_grad[5:]):
-            plan.live_forwards += 1
-        if _VALIDATE:
-            raise_on_device_errors()
-        return out
-
-    @staticmethod
-    def backward(ctx, g):
-        if not ctx.training:
-            raise PgnnError("backward through the eval-mode encoder is not implemented (SURVEY.md section 3.3)")
-        if getattr(ctx, "released", False):
-            raise PgnnError("the whole-encoder op released its workspace after its first backward: a second backward through the same "
-                            "graph (retain_graph) is not supported; set model.fused = False for that")
-        plan = ctx.plan
-        N, E, L, D = ctx.dims
-        g = _f32(g)
-
-        def run(flat):
-            check(lib.pgnn_chem_conv_backward(plan.conv, ctx.ptrs, _p(g), g.stride(0), _p(ctx.x), _p(ctx.ea), N, E, L, D, _precision,
-                                              _p(flat), _p(ctx.ws), ctx.wsb, _st()), "chem_conv_backward")
-        out = _deliver_flat_grads(plan, ctx, run)
-        _release_ctx(ctx)
-        return out
-
-
-def chem_conv_encoder(plan: ChemConvPlan, x, edge_index, edge_attr, training: bool):
-    return _ChemConvEncoder.apply(plan, x, edge_index, edge_attr, training, *plan.params)
 
 
 # ------------------------------------------------------------------------------------------------

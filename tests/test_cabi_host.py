@@ -1,5 +1,6 @@
 """CPU: the C-ABI library loads, exports every symbol include/pgnn_b200.h declares, validates arguments
 without touching a device, and the host-side modules keep the reference's state_dict contract."""
+import ctypes
 import importlib
 import os
 
@@ -30,6 +31,11 @@ def test_argument_validation_without_gpu():
     assert dll.pgnn_linear_fwd(None, 0, None, None, 0, 4, 3, 0, None, 0, 0, None) == 0    # M == 0: nothing to do
     assert dll.pgnn_aggregate_fwd(None, 0, None, None, 0, 0, 300, None, None, 0, None, None, 0, None, 0, None, 0, None) == 0
     assert dll.pgnn_aggregate_fwd(None, 0, None, None, 0, 5, 300, None, None, 7, None, None, 0, None, 0, None, 0, None) == -1
+    off = (ctypes.c_int64 * 64)()
+    for conv_type in (0, 4):   # 1..3 are GCN / GraphSAGE / GAT; GIN has entry points of its own
+        assert dll.pgnn_chem_conv_num_params(conv_type, 5) == -1
+        assert dll.pgnn_chem_conv_grad_offsets(conv_type, 5, 300, off) == -1
+        assert dll.pgnn_chem_conv_workspace_bytes(conv_type, 100, 200, 5, 300) == -1
     with pytest.raises(cabi.PgnnError):
         cabi.check(-4, "x")
 
@@ -43,9 +49,18 @@ def test_state_dict_contract(domain, t):
     assert set(model.state_dict().keys()) == set(P.keys())
     for k, v in model.state_dict().items():
         assert tuple(v.shape) == tuple(P[k].shape), k
-    assert sum(p.numel() for p in model.parameters()) == {
+    total = {
         ("chem", "gin"): 1857900, ("chem", "gcn"): 504900, ("chem", "graphsage"): 504900, ("chem", "gat"): 977400,
         ("bio", "gin"): 2726100, ("bio", "gcn"): 467100, ("bio", "graphsage"): 467100, ("bio", "gat"): 941100}[(domain, t)]
+    assert sum(p.numel() for p in model.parameters()) == total
+    if domain == "chem":
+        # the whole-encoder plan (host calls only): its flat gradient layout tiles [0, total) in parameter order
+        plan = model._fused_plan()
+        assert plan is not None and plan.gnn_type == t
+        assert sorted(map(id, plan.params)) == sorted(map(id, model.parameters()))
+        assert len(plan.offsets) == len(plan.params) + 1 and plan.offsets[0] == 0 and plan.offsets[-1] == plan.total == total
+        for i, p in enumerate(plan.params):
+            assert plan.offsets[i + 1] - plan.offsets[i] == p.numel(), i
 
 
 def test_shipped_checkpoints_load():

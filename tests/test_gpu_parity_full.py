@@ -32,7 +32,7 @@ def _compare(name, step, config, b, P, aux_fn, loss_fn=None):
     step.load_state(P)
     d = _dev(b)
     plan = getattr(getattr(step, "model", None), "_fused_plan", lambda: None)()
-    track = plan is not None and hasattr(plan, "keep_workspace") and config == "masking"
+    track = plan is not None and plan.gnn_type == "gin" and config == "masking"
     if track:
         plan.keep_workspace = True
     loss = step(d)
