@@ -190,6 +190,19 @@ PGNN_API int pgnn_bn_bwd(const float* gy, int64_t ldgy, const float* x, int64_t 
 PGNN_API int pgnn_relu_fwd(const float* x, int64_t ldx, int64_t M, int64_t C, float* y, int64_t ldy, void* stream);
 PGNN_API int pgnn_relu_bwd(const float* gy, int64_t ldgy, const float* y, int64_t ldy_, int64_t M, int64_t C,
                            float* gx, int64_t ldgx, void* stream);
+/* Dropout (chem/model.py:271-275, bio/model.py:283-286: F.dropout(h, p, training=True)) with a DEFINED draw: element (row i,
+ * column c) of layer `layer`'s [M, C] activation is kept iff
+ *     r = splitmix64(seed, ((uint64)layer << 40) | (uint64)(i * C + c)) >> 32   (a uint32; splitmix64 as in pgnn_mask_atoms)
+ *     r >= thr,   thr = floor(p * 2^32) for 0 <= p < 1;  p == 1 drops everything
+ * and y = x * (kept ? scale : 0.f) with scale = (float)(1.0 / (1.0 - p)) (p as the float passed here).  A dropped NaN stays NaN and
+ * a dropped +-Inf becomes NaN, as torch's x * mask * scale does.  The mask is a pure function of (seed, layer, i, c): the backward
+ * gx = gy * (kept ? scale : 0.f) regenerates it, and no mask tensor exists.  torch's Philox stream cannot be matched, so the draw
+ * is defined here (as for pgnn_mask_atoms); the distribution is the same.  0 <= layer < 2^24, M * C < 2^40; p outside [0, 1] or
+ * NaN is PGNN_EINVAL. */
+PGNN_API int pgnn_dropout_fwd(const float* x, int64_t ldx, int64_t M, int64_t C, float p, int64_t seed, int64_t layer, float* y,
+                              int64_t ldy, void* stream);
+PGNN_API int pgnn_dropout_bwd(const float* gy, int64_t ldgy, int64_t M, int64_t C, float p, int64_t seed, int64_t layer, float* gx,
+                              int64_t ldgx, void* stream);
 /* GraphSAGE update: y = x / max(||x||_2, 1e-12) per row (chem/model.py:201-202) and its backward */
 PGNN_API int pgnn_l2norm_fwd(const float* x, int64_t ldx, int64_t M, int64_t C, float* y, int64_t ldy,
                              float* norm /*[M]*/, void* stream);
@@ -260,7 +273,8 @@ PGNN_API int pgnn_bce_logits_fwd(const float* logits, int64_t ld, int64_t M, int
                                  void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Whole-encoder entry points: chem GNN with gnn_type="gin", JK="last", drop_ratio=0 (chem/model.py:255-290).
+ * Whole-encoder entry points: chem GNN with gnn_type="gin", JK="last" (chem/model.py:255-290).  pgnn_chem_gin_* run without
+ * dropout; pgnn_chem_encoder_forward / _backward below are the same path for every gnn_type with live dropout.
  * What GNN.forward / loss.backward() bind to: two boundary crossings per training step.
  *
  * params: HOST array of num_params = 2 + 8*L DEVICE pointers in state_dict order
@@ -333,6 +347,26 @@ PGNN_API int pgnn_chem_conv_forward(int conv_type, const void* const* params, vo
 PGNN_API int pgnn_chem_conv_backward(int conv_type, const void* const* params, const float* g_node_rep, int64_t ldg,
                                      const int64_t* x, const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D,
                                      int precision, float* grads, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* The one implementation behind pgnn_chem_gin_* (gnn_type 0) and pgnn_chem_conv_* (gnn_type = PGNN_CONV_*), with the reference's
+ * dropout (chem/model.py:271-275): in training mode with drop_p > 0, layer l's output (after its BatchNorm and, except for the
+ * last layer, its ReLU) is multiplied by the pgnn_dropout_fwd mask of (drop_p, drop_seed, layer = l).  It never makes a pass of
+ * its own: the kernel that writes or loads layer l's output applies it (GIN: the next layer's gather and the BatchNorm apply of
+ * node_rep; the conv types: the BatchNorm apply that writes the layer's output), and the backward applies it to the incoming
+ * gradient inside the BatchNorm backward.  Eval mode (training = 0) applies none; backward must get the forward's drop_p and
+ * drop_seed.  drop_p == 0 is exactly pgnn_chem_gin_* / pgnn_chem_conv_*, which pass it.  Workspace, parameter and gradient
+ * layouts are those of the type's own entry points; backward's edge_attr is only read for GAT.  gnn_type outside {0, 1, 2, 3},
+ * drop_p outside [0, 1] or NaN: PGNN_EINVAL. */
+PGNN_API int pgnn_chem_encoder_forward(int gnn_type, const void* const* params, void* const* bn_running_mean,
+                                       void* const* bn_running_var, void* const* bn_num_batches_tracked, const int64_t* x,
+                                       const int64_t* edge_index, const int64_t* edge_attr, int64_t N, int64_t E, int64_t L,
+                                       int64_t D, int training, float momentum, float eps, float drop_p, int64_t drop_seed,
+                                       int precision, float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes,
+                                       void* stream);
+PGNN_API int pgnn_chem_encoder_backward(int gnn_type, const void* const* params, const float* g_node_rep, int64_t ldg,
+                                        const int64_t* x, const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D,
+                                        float drop_p, int64_t drop_seed, int precision, float* grads, void* workspace,
+                                        int64_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Either side of the path inside a training step (SURVEY.md section 8(f): f1 collation, f2 optimizer).

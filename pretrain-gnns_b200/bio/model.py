@@ -11,7 +11,6 @@ Because the message is linear in e_ij, `Linear(9, .)` is applied once per NODE t
 not once per edge: the reference's [E+N, 600] message tensor (845 MB at B=64) never exists.
 """
 import torch
-import torch.nn.functional as F
 from torch import nn
 
 from .. import ops
@@ -135,14 +134,16 @@ class GNN(nn.Module):
 
     def forward(self, x, edge_index, edge_attr):
         graph = ops.graph_for(edge_index, x.size(0))
+        drop = self.training and self.drop_ratio > 0
+        seed = ops.draw_seed() if drop else 0  # one per forward; layer l's mask is ops.dropout's of (seed, l)
         h = x
         hs = []
         for l, conv in enumerate(self.gnns):
             h = conv(h, edge_index, edge_attr, graph=graph)
             if l != self.num_layer - 1:
                 h = ops.relu(h)
-            if self.drop_ratio > 0:
-                h = F.dropout(h, self.drop_ratio, training=self.training)
+            if drop:
+                h = ops.dropout(h, self.drop_ratio, seed, l)
             hs.append(h)
         if self.JK == "last":
             return hs[-1]

@@ -13,7 +13,6 @@ is underneath: no torch_geometric, no per-edge tensors.  Each batch is bucketed 
 embedding sum is folded into a per-node 9-bin summary, and every op is a CUDA kernel behind the C ABI.
 """
 import torch
-import torch.nn.functional as F
 from torch import nn
 
 from .. import ops
@@ -153,9 +152,9 @@ class GNN(nn.Module):
     _DEFAULT_AGGR = {"gin": "add", "gcn": "add", "gat": "add", "graphsage": "mean"}
 
     def _fused_plan(self):
-        """The whole-encoder kernels (pgnn_chem_gin_* / pgnn_chem_conv_*) cover every gnn_type with JK='last', the conv's
-        default aggregation (and GAT's 2 heads / slope 0.2) and no live dropout."""
-        if not (self.fused and self.JK == "last" and (self.drop_ratio == 0 or not self.training)):
+        """The whole-encoder kernels (pgnn_chem_encoder_*) cover every gnn_type with JK='last', the conv's default aggregation
+        (and GAT's 2 heads / slope 0.2), with or without dropout."""
+        if not (self.fused and self.JK == "last"):
             return None
         if any(conv.aggr != self._DEFAULT_AGGR[self._gnn_type] for conv in self.gnns) or any(bn.training != self.training for bn in self.batch_norms):
             return None
@@ -172,9 +171,13 @@ class GNN(nn.Module):
             x, edge_index, edge_attr = argv[0].x, argv[0].edge_index, argv[0].edge_attr
         else:
             raise ValueError("unmatched number of arguments.")
+        # one dropout seed per forward, drawn on the host only when dropout is live (the RNG stream is untouched otherwise); both
+        # paths below derive layer l's mask from (seed, l), so under the same torch.manual_seed they drop the same units
+        drop = self.training and self.drop_ratio > 0
+        seed = ops.draw_seed() if drop else 0
         plan = self._fused_plan()
         if plan is not None:
-            return ops.chem_encoder(plan, x, edge_index, edge_attr, self.training)
+            return ops.chem_encoder(plan, x, edge_index, edge_attr, self.training, self.drop_ratio if drop else 0.0, seed)
         graph = ops.graph_for(edge_index, x.size(0))
         h = ops.chem_embed(x, self.x_embedding1.weight, self.x_embedding2.weight)
         hs = [h]
@@ -182,8 +185,8 @@ class GNN(nn.Module):
         for l, (conv, bn) in enumerate(zip(self.gnns, self.batch_norms)):
             h = conv(h, edge_index, edge_attr, graph=graph)
             h = ops.batch_norm(h, bn, relu=(l != last))        # BN + ReLU fused (chem/model.py:269-275)
-            if self.drop_ratio > 0:
-                h = F.dropout(h, self.drop_ratio, training=self.training)
+            if drop:
+                h = ops.dropout(h, self.drop_ratio, seed, l)
             hs.append(h)
         if self.JK == "last":
             return hs[-1]

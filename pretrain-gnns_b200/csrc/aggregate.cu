@@ -49,12 +49,16 @@ __device__ __forceinline__ void add4(float4& acc, float4 v) {
   acc.w = __fadd_rn(acc.w, v.w);
 }
 
-__global__ void __launch_bounds__(256)
-k_aggregate_fwd(const float* __restrict__ x, int64_t ldx, const float* __restrict__ in_scale,
-                const float* __restrict__ in_shift, int in_relu, int64_t n, int C4, const int* __restrict__ rowptr,
-                const int* __restrict__ nbr, int mode, const float* __restrict__ dinv, const float* __restrict__ S, int Q,
-                const float* __restrict__ T, const float* __restrict__ T2, int q_split, int64_t edge_off, float* __restrict__ out,
-                int64_t ldo, PgnnBnFold fold) {
+// DROP: every loaded row j is also multiplied by the dropout mask of (drop.layer, j, c) after the affine + ReLU, i.e. the gather
+// reads the previous layer's dropout output without it ever being written (k_aggregate_fwd_drop; k_aggregate_fwd has no mask).
+template <bool DROP>
+__device__ __forceinline__ void aggregate_fwd_body(const float* __restrict__ x, int64_t ldx, const float* __restrict__ in_scale,
+                                                   const float* __restrict__ in_shift, int in_relu, int64_t n, int C4,
+                                                   const int* __restrict__ rowptr, const int* __restrict__ nbr, int mode,
+                                                   const float* __restrict__ dinv, const float* __restrict__ S, int Q,
+                                                   const float* __restrict__ T, const float* __restrict__ T2, int q_split,
+                                                   int64_t edge_off, float* __restrict__ out, int64_t ldo, const PgnnBnFold& fold,
+                                                   const PgnnDropout& drop) {
   pdl_prologue();
   const int64_t total = n * C4;
   const int C = C4 * 4;
@@ -69,14 +73,20 @@ k_aggregate_fwd(const float* __restrict__ x, int64_t ldx, const float* __restric
     const int i = (int)(idx / C4);
     const int c = (int)(idx - (int64_t)i * C4) * 4;
     const int lo = rowptr[i], hi = rowptr[i + 1];
+    // the effective input row j at columns c..c+3: act(x * in_scale + in_shift), times the mask under DROP
+    auto act = [&](float4 v, int j) {
+      v = affine_act(v, in_scale, in_shift, c, in_relu);
+      if (DROP) v = dropout4(v, drop, j, C, c);
+      return v;
+    };
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     if (mode == PGNN_AGG_GCN) {
       const float di = dinv[i];
       for (int k = lo; k < hi; ++k) {
         const int s = nbr[k];
-        axpy4(acc, __fmul_rn(di, dinv[s]), affine_act(ld4(x + (int64_t)s * ldx + c), in_scale, in_shift, c, in_relu));
+        axpy4(acc, __fmul_rn(di, dinv[s]), act(ld4(x + (int64_t)s * ldx + c), s));
       }
-      axpy4(acc, __fmul_rn(di, di), affine_act(ld4(x + (int64_t)i * ldx + c), in_scale, in_shift, c, in_relu));
+      axpy4(acc, __fmul_rn(di, di), act(ld4(x + (int64_t)i * ldx + c), i));
     } else {
       // the self-loop row and up to four neighbour rows are in flight together (the chain rowptr -> nbr -> row is three
       // dependent L2 round trips per thread: memory-level parallelism, not bandwidth, bounds this kernel); the additions keep
@@ -89,21 +99,24 @@ k_aggregate_fwd(const float* __restrict__ x, int64_t ldx, const float* __restric
         const float4 v1 = ld4(x + (int64_t)s1 * ldx + c);
         const float4 v2 = ld4(x + (int64_t)s2 * ldx + c);
         const float4 v3 = ld4(x + (int64_t)s3 * ldx + c);
-        add4(acc, affine_act(v0, in_scale, in_shift, c, in_relu));
-        add4(acc, affine_act(v1, in_scale, in_shift, c, in_relu));
-        add4(acc, affine_act(v2, in_scale, in_shift, c, in_relu));
-        add4(acc, affine_act(v3, in_scale, in_shift, c, in_relu));
+        add4(acc, act(v0, s0));
+        add4(acc, act(v1, s1));
+        add4(acc, act(v2, s2));
+        add4(acc, act(v3, s3));
       }
       if (k + 1 < hi) {
         const int s0 = nbr[k], s1 = nbr[k + 1];
         const float4 v0 = ld4(x + (int64_t)s0 * ldx + c);
         const float4 v1 = ld4(x + (int64_t)s1 * ldx + c);
-        add4(acc, affine_act(v0, in_scale, in_shift, c, in_relu));
-        add4(acc, affine_act(v1, in_scale, in_shift, c, in_relu));
+        add4(acc, act(v0, s0));
+        add4(acc, act(v1, s1));
         k += 2;
       }
-      if (k < hi) add4(acc, affine_act(ld4(x + (int64_t)nbr[k] * ldx + c), in_scale, in_shift, c, in_relu));
-      add4(acc, affine_act(vself, in_scale, in_shift, c, in_relu));  // self-loop last
+      if (k < hi) {
+        const int s0 = nbr[k];
+        add4(acc, act(ld4(x + (int64_t)s0 * ldx + c), s0));
+      }
+      add4(acc, act(vself, i));  // self-loop last
       if (mode == PGNN_AGG_MEAN) {
         const float cnt = (float)(hi - lo + 1);
         acc.x = __fdiv_rn(acc.x, cnt);
@@ -133,6 +146,24 @@ k_aggregate_fwd(const float* __restrict__ x, int64_t ldx, const float* __restric
       st4(out + (int64_t)i * ldo + edge_off + c, e);
     }
   }
+}
+__global__ void __launch_bounds__(256)
+k_aggregate_fwd(const float* __restrict__ x, int64_t ldx, const float* __restrict__ in_scale,
+                const float* __restrict__ in_shift, int in_relu, int64_t n, int C4, const int* __restrict__ rowptr,
+                const int* __restrict__ nbr, int mode, const float* __restrict__ dinv, const float* __restrict__ S, int Q,
+                const float* __restrict__ T, const float* __restrict__ T2, int q_split, int64_t edge_off, float* __restrict__ out,
+                int64_t ldo, PgnnBnFold fold) {
+  aggregate_fwd_body<false>(x, ldx, in_scale, in_shift, in_relu, n, C4, rowptr, nbr, mode, dinv, S, Q, T, T2, q_split, edge_off, out, ldo,
+                            fold, PgnnDropout{});
+}
+__global__ void __launch_bounds__(256)
+k_aggregate_fwd_drop(const float* __restrict__ x, int64_t ldx, const float* __restrict__ in_scale,
+                     const float* __restrict__ in_shift, int in_relu, int64_t n, int C4, const int* __restrict__ rowptr,
+                     const int* __restrict__ nbr, int mode, const float* __restrict__ dinv, const float* __restrict__ S, int Q,
+                     const float* __restrict__ T, const float* __restrict__ T2, int q_split, int64_t edge_off, float* __restrict__ out,
+                     int64_t ldo, PgnnBnFold fold, PgnnDropout drop) {
+  aggregate_fwd_body<true>(x, ldx, in_scale, in_shift, in_relu, n, C4, rowptr, nbr, mode, dinv, S, Q, T, T2, q_split, edge_off, out, ldo,
+                           fold, drop);
 }
 
 __global__ void __launch_bounds__(256)
@@ -454,15 +485,20 @@ int pgnn_internal_edge_table_bwd(const float* S, int Q, const float* g, int64_t 
 int pgnn_internal_aggregate_fwd(const float* x, int64_t ldx, const float* in_scale, const float* in_shift, int in_relu,
                                 int64_t num_nodes, int64_t C, const int32_t* rowptr_t, const int32_t* nbr_t, int mode, const float* dinv,
                                 const float* S, int64_t Q, const float* T, const float* T2, int q_split, int64_t edge_off, float* out,
-                                int64_t ldo, cudaStream_t st, const PgnnBnFold* fold) {
+                                int64_t ldo, cudaStream_t st, const PgnnBnFold* fold, const PgnnDropout* drop) {
   if (num_nodes == 0) return PGNN_OK;
   if (C % 4 || ldx % 4 || ldo % 4 || !aligned16(x) || !aligned16(out) || (T && !aligned16(T)) || (T2 && !aligned16(T2)) ||
       (in_scale && (!aligned16(in_scale) || !aligned16(in_shift))))
     return PGNN_EUNSUPPORTED;
   const int C4 = (int)(C / 4);
-  PGNN_CUDA(pgnn_launch(k_aggregate_fwd, dim3(grid_items(num_nodes * C4, 256)), dim3(256), fold ? sizeof(float) * 2 * C : 0, st, x, ldx, in_scale,
-                        in_shift, in_relu, num_nodes, C4, rowptr_t, nbr_t, mode, dinv, S, (int)Q, T, T2, q_split, edge_off, out, ldo,
-                        fold ? *fold : PgnnBnFold{}));
+  if (drop && drop->p > 0.f)
+    PGNN_CUDA(pgnn_launch(k_aggregate_fwd_drop, dim3(grid_items(num_nodes * C4, 256)), dim3(256), fold ? sizeof(float) * 2 * C : 0, st, x, ldx,
+                          in_scale, in_shift, in_relu, num_nodes, C4, rowptr_t, nbr_t, mode, dinv, S, (int)Q, T, T2, q_split, edge_off, out,
+                          ldo, fold ? *fold : PgnnBnFold{}, *drop));
+  else
+    PGNN_CUDA(pgnn_launch(k_aggregate_fwd, dim3(grid_items(num_nodes * C4, 256)), dim3(256), fold ? sizeof(float) * 2 * C : 0, st, x, ldx, in_scale,
+                          in_shift, in_relu, num_nodes, C4, rowptr_t, nbr_t, mode, dinv, S, (int)Q, T, T2, q_split, edge_off, out, ldo,
+                          fold ? *fold : PgnnBnFold{}));
   PGNN_LAUNCH_CHECK();
   return PGNN_OK;
 }
@@ -489,7 +525,7 @@ int pgnn_aggregate_fwd(const float* x, int64_t ldx, const float* in_scale, const
   PGNN_CHECK_ARG(!S || (T && Q > 0 && Q <= kMaxQ));
   PGNN_CHECK_ARG(edge_off == 0 || (S && edge_off % 4 == 0));
   return pgnn_internal_aggregate_fwd(x, ldx, in_scale, in_shift, in_relu, num_nodes, C, rowptr_t, nbr_t, mode, dinv, S, Q, T, nullptr,
-                                     (int)Q, edge_off, out, ldo, as_stream(stream), nullptr);
+                                     (int)Q, edge_off, out, ldo, as_stream(stream), nullptr, nullptr);
 }
 
 int pgnn_aggregate_bwd(const float* g, int64_t ldg, int64_t num_nodes, int64_t C, const int32_t* rowptr_s,

@@ -102,6 +102,53 @@ __device__ __forceinline__ void bn_fold_column(const PgnnBnFold& f, int C, int c
   }
 }
 
+// The library's one counter-based hash: the 64-bit key of position `idx` under `seed`.  MaskAtom / MaskEdge / the context root
+// draw (transforms.cu, mask_edges.cu, extract.cu) and dropout (below) all draw through it; oracle/step_io_oracle.py and the
+// dropout tests restate it.
+__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t seed, uint64_t idx) {
+  uint64_t z = seed + (idx + 1ull) * 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+// Dropout of layer `layer`'s [rows, C] activation (include/pgnn_b200.h, pgnn_dropout_fwd): element (row i, column c) is kept
+// iff (splitmix64(seed, (layer << 40) | (i * C + c)) >> 32) >= thr, and then scaled by `scale`; a dropped element is multiplied
+// by 0 (so a dropped NaN / Inf gives NaN, as torch's x * mask * scale does).  The mask is regenerated wherever it is needed
+// (forward, backward, on load in the next layer's gather): no mask tensor exists.
+struct PgnnDropout {
+  float p = 0.f;
+  int64_t seed = 0;
+  int64_t layer = 0;
+  uint64_t thr = 0;   // floor(p * 2^32); 2^32 for p == 1 (no 32-bit draw reaches it: everything is dropped)
+  float scale = 1.f;  // (float)(1 / (1 - p)); 0 for p == 1
+};
+
+// host: the dropout of (p, seed, layer); false for p outside [0, 1] or NaN
+static inline bool pgnn_make_dropout(float p, int64_t seed, int64_t layer, PgnnDropout* d) {
+  if (!(p >= 0.f && p <= 1.f)) return false;
+  d->p = p;
+  d->seed = seed;
+  d->layer = layer;
+  d->thr = p == 1.f ? (1ull << 32) : (uint64_t)((double)p * 4294967296.0);
+  d->scale = p == 1.f ? 0.f : (float)(1.0 / (1.0 - (double)p));
+  return true;
+}
+
+// the factor element (row, c) of a [*, C] activation is multiplied by: `scale` if kept, else 0
+__device__ __forceinline__ float dropout_factor(const PgnnDropout& d, int64_t row, int64_t C, int64_t c) {
+  const uint64_t idx = ((uint64_t)d.layer << 40) | (uint64_t)(row * C + c);
+  const uint64_t r = splitmix64((uint64_t)d.seed, idx) >> 32;
+  return r >= d.thr ? d.scale : 0.f;
+}
+__device__ __forceinline__ float4 dropout4(float4 v, const PgnnDropout& d, int64_t row, int64_t C, int64_t c) {
+  v.x *= dropout_factor(d, row, C, c);
+  v.y *= dropout_factor(d, row, C, c + 1);
+  v.z *= dropout_factor(d, row, C, c + 2);
+  v.w *= dropout_factor(d, row, C, c + 3);
+  return v;
+}
+
 // Epilogue of the tensor-core GEMM kernel (dense_tc.cu)
 struct TcEpilogue {
   const float* bias;      // [N] or null

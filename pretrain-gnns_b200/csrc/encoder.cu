@@ -1,4 +1,4 @@
-// Whole-encoder entry points for the chem GNN (chem/model.py:206-290 with JK="last", drop_ratio=0): ONE call enqueues graph
+// Whole-encoder entry points for the chem GNN (chem/model.py:206-290 with JK="last", any drop_ratio): ONE call enqueues graph
 // preparation, the atom embedding and all L layers; a second call enqueues the whole backward.  This is what GNN.forward binds
 // to, so a training step crosses the Python/C boundary twice instead of ~60 (GIN) or ~100 (conv types) times, without the
 // per-op allocations and the torch.cat of the two bond tables per layer and pass.
@@ -12,6 +12,12 @@
 //   GAT        (chem/model.py:134-165):  xl = Linear(D,2D)(h); out_i = mean_heads(sum_j alpha_ij (xl_j + e_ij)) + bias
 //   each followed by BatchNorm1d(D) and, except after the last layer, ReLU (chem/model.py:267-276).  The per-layer arithmetic
 //   is the operator-level C ABI of include/pgnn_b200.h (the same kernels the layer-by-layer Python composition launches).
+//
+// Dropout (training, drop_p > 0; chem/model.py:271-275) never makes a pass of its own either: layer l's mask (PgnnDropout with
+// layer = l, common.cuh) is applied by whichever kernel materialises or loads layer l's output -- GIN: the next layer's gather
+// and, for the last layer, the BatchNorm apply that writes node_rep; the conv types: the BatchNorm apply that writes hout.  The
+// backward applies it to the incoming gradient inside the BatchNorm backward.  drop_p == 0 launches exactly the kernels without
+// a mask.
 //
 // Parameters arrive as a host array of device pointers in a fixed order, gradients leave in ONE flat fp32 buffer with the
 // library-defined layout of pgnn_chem_gin_grad_offsets / pgnn_chem_conv_grad_offsets (grad_layout below), which is also the
@@ -27,7 +33,7 @@ int pgnn_internal_edge_table_bwd2(const float* S, int Q, const float* g, int64_t
 int pgnn_internal_aggregate_fwd(const float* x, int64_t ldx, const float* in_scale, const float* in_shift, int in_relu,
                                 int64_t num_nodes, int64_t C, const int32_t* rowptr_t, const int32_t* nbr_t, int mode, const float* dinv,
                                 const float* S, int64_t Q, const float* T, const float* T2, int q_split, int64_t edge_off, float* out,
-                                int64_t ldo, cudaStream_t st, const PgnnBnFold* fold);
+                                int64_t ldo, cudaStream_t st, const PgnnBnFold* fold, const PgnnDropout* drop);
 
 int pgnn_internal_chem_onehot(const int64_t* x, int64_t n, int rows1, int rows2, float* onehot, int64_t ld, cudaStream_t st);
 
@@ -44,10 +50,18 @@ int pgnn_tc_linear_bwd_x_wt(const float* gy, int64_t ldgy, const float* wT, int6
 int pgnn_internal_transpose_batch(int count, const float* const* in, float* const* out, const int* rows, const int* cols,
                                   cudaStream_t st);
 int pgnn_internal_bn_apply_fold(const float* x, int64_t ldx, int64_t M, int64_t C, const PgnnBnFold& fold, int relu, float* y,
-                                int64_t ldy, cudaStream_t st);
+                                int64_t ldy, cudaStream_t st, const PgnnDropout* drop);
 int pgnn_internal_bn_bwd_colsum(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma,
                                 const float* beta, const float* save_mean, const float* save_invstd, int relu, float* gx,
-                                int64_t ldgx, float* ggamma, float* gbeta, float* colsum, void* workspace, cudaStream_t st);
+                                int64_t ldgx, float* ggamma, float* gbeta, float* colsum, void* workspace, cudaStream_t st,
+                                const PgnnDropout* drop);
+int pgnn_internal_bn_fwd_train(const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma, const float* beta,
+                               float* running_mean, float* running_var, int64_t* num_batches_tracked, float momentum, float eps,
+                               int relu, float* y, int64_t ldy, float* save_mean, float* save_invstd, float* scale, float* shift,
+                               void* workspace, int64_t workspace_bytes, void* stream, const PgnnDropout* drop);
+int pgnn_internal_bn_bwd(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma,
+                         const float* beta, const float* save_mean, const float* save_invstd, int relu, float* gx, int64_t ldgx,
+                         float* ggamma, float* gbeta, void* workspace, int64_t workspace_bytes, void* stream, const PgnnDropout* drop);
 
 namespace {
 
@@ -67,6 +81,18 @@ enum { A_W = 0, A_B, A_ATT, A_BIAS, A_ET1, A_ET2, A_GAMMA, A_BETA, A_COUNT };   
 inline int layer_params(int type) { return type == kGin ? L_COUNT : type == PGNN_CONV_GAT ? A_COUNT : G_COUNT; }
 inline int agg_mode(int type) { return type == kGin ? PGNN_AGG_SUM : type == PGNN_CONV_GCN ? PGNN_AGG_GCN : PGNN_AGG_MEAN; }
 bool valid_conv(int t) { return t == PGNN_CONV_GCN || t == PGNN_CONV_SAGE || t == PGNN_CONV_GAT; }
+
+// Per-layer dropout of one pass: layer l's mask is PgnnDropout(p, seed, l).  p == 0 (or eval mode) leaves every layer without
+// one, so the kernels without a mask run.
+struct Drops {
+  float p = 0.f;
+  int64_t seed = 0;
+  PgnnDropout at(int64_t l) const {
+    PgnnDropout d;
+    pgnn_make_dropout(p, seed, l, &d);
+    return d;
+  }
+};
 
 #define TRY(call)                     \
   do {                                \
@@ -309,44 +335,10 @@ int embed_backward(const SideCtx* sc, const Front& f, const float* gh, const int
   return rc;
 }
 
-}  // namespace
-
-extern "C" {
-
-// ------------------------------------------------------------------------------------------------------------------------------
-// GIN
-// ------------------------------------------------------------------------------------------------------------------------------
-int64_t pgnn_chem_gin_num_params(int64_t L) { return L < 1 ? PGNN_EINVAL : grad_layout(kGin, L, 0, nullptr); }
-
-int pgnn_chem_gin_grad_offsets(int64_t L, int64_t D, int64_t* offsets /*host [num_params + 1]*/) {
-  PGNN_CHECK_ARG(L >= 1 && D > 0 && offsets);
-  grad_layout(kGin, L, D, offsets);
-  return PGNN_OK;
-}
-
-int64_t pgnn_chem_gin_workspace_bytes(int64_t N, int64_t E, int64_t L, int64_t D) {
-  if (N < 0 || E < 0 || L < 1 || D <= 0) return PGNN_EINVAL;
-  return carve_gin(nullptr, N, E, L, D).total;
-}
-
-// Development / test aid: byte offsets inside the workspace of the saved activations a test needs to reconstruct the
-// ReLU decisions the encoder actually took: out[0] = z1 (post-ReLU hidden activations, [L][N][2D]), out[1] = z2 (pre-BatchNorm
-// layer outputs, [L][N][D]), out[2] = BatchNorm batch mean [L][D], out[3] = invstd [L][D].
-int pgnn_chem_gin_debug_layout(int64_t N, int64_t E, int64_t L, int64_t D, int64_t* out4) {
-  PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && out4);
-  char* base = reinterpret_cast<char*>(0x1000);  // carve_gin() only does pointer arithmetic
-  GinWs w = carve_gin(base, N, E, L, D);
-  out4[0] = reinterpret_cast<char*>(w.z1) - base;
-  out4[1] = reinterpret_cast<char*>(w.z2) - base;
-  out4[2] = reinterpret_cast<char*>(w.mean) - base;
-  out4[3] = reinterpret_cast<char*>(w.invstd) - base;
-  return PGNN_OK;
-}
-
-int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
-                          void* const* bn_num_batches_tracked, const int64_t* x, const int64_t* edge_index,
-                          const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, int training, float momentum, float eps,
-                          int precision, float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes, void* stream) {
+int gin_forward(const void* const* params, void* const* bn_running_mean, void* const* bn_running_var, void* const* bn_num_batches_tracked,
+                const int64_t* x, const int64_t* edge_index, const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D,
+                int training, float momentum, float eps, const Drops& drops, int precision, float* node_rep, int64_t ld_out,
+                void* workspace, int64_t workspace_bytes, void* stream) {
   PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && bn_running_mean && bn_running_var && workspace);
   PGNN_CHECK_ARG(N == 0 || (x && node_rep));
   if (workspace_bytes < pgnn_chem_gin_workspace_bytes(N, E, L, D)) return PGNN_EWORKSPACE;
@@ -364,10 +356,11 @@ int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mea
     float* z1 = w.z1 + l * N * 2 * D;
     float* z2 = w.z2 + l * N * D;
     const bool last = (l == L - 1);
-    // gather (the previous layer's BatchNorm + ReLU applied on load) + GEMM1
+    const PgnnDropout drop_in = drops.at(l > 0 ? l - 1 : 0), drop_out = drops.at(l);  // the previous layer's mask, this layer's
+    // gather (the previous layer's BatchNorm + ReLU + dropout applied on load) + GEMM1
     TRY(pgnn_internal_aggregate_fwd(h, D, in_scale, in_shift, in_scale != nullptr || have_fold, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_SUM,
                                     nullptr, w.S, 9, (const float*)p[L_ET1], (const float*)p[L_ET2], 6, 0, aggr, D, as_stream(stream),
-                                    have_fold ? &fold : nullptr));
+                                    have_fold ? &fold : nullptr, l > 0 ? &drop_in : nullptr));
     TRY(pgnn_linear_fwd(aggr, D, (const float*)p[L_W1], (const float*)p[L_B1], N, 2 * D, D, 1, z1, 2 * D, precision, stream));
     have_fold = false;
     // GEMM2; on the tensor path its epilogue also accumulates the BatchNorm batch statistics of z2 (fp64 atomics)
@@ -392,7 +385,7 @@ int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mea
       fold.save_mean = w.mean + l * D; fold.save_invstd = w.invstd + l * D;
       fold.momentum = momentum; fold.eps = eps; fold.set_rows((int)N);
       if (last) {
-        TRY(pgnn_internal_bn_apply_fold(z2, D, N, D, fold, 0, node_rep, ld_out, as_stream(stream)));
+        TRY(pgnn_internal_bn_apply_fold(z2, D, N, D, fold, 0, node_rep, ld_out, as_stream(stream), &drop_out));
       } else {
         have_fold = true;
       }
@@ -400,10 +393,10 @@ int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mea
       in_scale = in_shift = nullptr;
     } else if (training) {
       // statistics only for inner layers (applied on load by the next gather); the last layer materialises node_rep
-      TRY(pgnn_bn_fwd_train(z2, D, N, D, (const float*)p[L_GAMMA], (const float*)p[L_BETA], (float*)bn_running_mean[l],
-                            (float*)bn_running_var[l], bn_num_batches_tracked ? (int64_t*)bn_num_batches_tracked[l] : nullptr, momentum,
-                            eps, 0, last ? node_rep : nullptr, ld_out, w.mean + l * D, w.invstd + l * D, w.scale + l * D,
-                            w.shift + l * D, w.scratch, w.scratch_bytes, stream));
+      TRY(pgnn_internal_bn_fwd_train(z2, D, N, D, (const float*)p[L_GAMMA], (const float*)p[L_BETA], (float*)bn_running_mean[l],
+                                     (float*)bn_running_var[l], bn_num_batches_tracked ? (int64_t*)bn_num_batches_tracked[l] : nullptr,
+                                     momentum, eps, 0, last ? node_rep : nullptr, ld_out, w.mean + l * D, w.invstd + l * D, w.scale + l * D,
+                                     w.shift + l * D, w.scratch, w.scratch_bytes, stream, &drop_out));
       h = z2;
       in_scale = w.scale + l * D;
       in_shift = w.shift + l * D;
@@ -419,9 +412,8 @@ int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mea
   return PGNN_OK;
 }
 
-int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x, int64_t N, int64_t E,
-                           int64_t L, int64_t D, int precision, float* grads, void* workspace, int64_t workspace_bytes,
-                           void* stream) {
+int gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x, int64_t N, int64_t E, int64_t L,
+                 int64_t D, const Drops& drops, int precision, float* grads, void* workspace, int64_t workspace_bytes, void* stream) {
   PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && grads && workspace);
   if (workspace_bytes < pgnn_chem_gin_workspace_bytes(N, E, L, D)) return PGNN_EWORKSPACE;
   int64_t off[2 + L_COUNT * 64 + 1];
@@ -464,11 +456,13 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
     const int par = (int)(l & 1);
     float* gz2 = w.gz2 + (sc ? par * N * D : 0);
     float* gz1 = w.gz1 + (sc ? par * N * 2 * D : 0);
-    // BatchNorm (+ReLU mask recomputed from z2) backward; the same pass leaves colsum(gz2) = gradient of mlp.2.bias
+    // BatchNorm (dropout mask regenerated, ReLU mask recomputed from z2) backward; the same pass leaves colsum(gz2) = gradient
+    // of mlp.2.bias
     if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad2 has finished reading this copy
+    const PgnnDropout drop = drops.at(l);
     TRY(pgnn_internal_bn_bwd_colsum(gy, ldgy, z2, D, N, D, (const float*)p[L_GAMMA], (const float*)p[L_BETA], w.mean + l * D,
                                     w.invstd + l * D, !last, gz2, D, grads + o[L_GAMMA], grads + o[L_BETA], grads + o[L_B2],
-                                    w.scratch, st));
+                                    w.scratch, st, &drop));
     // MLP backward.  On the tensor path the dgrad epilogues carry the column reductions that would otherwise be
     // passes of their own: colsum(gz1) = gradient of mlp.0.bias, and S^T gaggr = gradient of the two bond tables.
     bool fused = false;
@@ -529,29 +523,10 @@ int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, i
   return embed_backward(sc, w, w.gh, x, N, D, precision, grads, off, w.wpart, w.wpart_floats, st);
 }
 
-// ------------------------------------------------------------------------------------------------------------------------------
-// GCN / GraphSAGE / GAT
-// ------------------------------------------------------------------------------------------------------------------------------
-int64_t pgnn_chem_conv_num_params(int conv_type, int64_t L) {
-  if (!valid_conv(conv_type) || L < 1) return PGNN_EINVAL;
-  return grad_layout(conv_type, L, 0, nullptr);
-}
-
-int pgnn_chem_conv_grad_offsets(int conv_type, int64_t L, int64_t D, int64_t* offsets) {
-  PGNN_CHECK_ARG(valid_conv(conv_type) && L >= 1 && D > 0 && offsets);
-  grad_layout(conv_type, L, D, offsets);
-  return PGNN_OK;
-}
-
-int64_t pgnn_chem_conv_workspace_bytes(int conv_type, int64_t N, int64_t E, int64_t L, int64_t D) {
-  if (!valid_conv(conv_type) || N < 0 || E < 0 || L < 1 || D <= 0) return PGNN_EINVAL;
-  return carve_conv(nullptr, conv_type, N, E, L, D).total;
-}
-
-int pgnn_chem_conv_forward(int conv_type, const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
-                           void* const* bn_num_batches_tracked, const int64_t* x, const int64_t* edge_index, const int64_t* edge_attr,
-                           int64_t N, int64_t E, int64_t L, int64_t D, int training, float momentum, float eps, int precision,
-                           float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes, void* stream) {
+int conv_forward(int conv_type, const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
+                 void* const* bn_num_batches_tracked, const int64_t* x, const int64_t* edge_index, const int64_t* edge_attr, int64_t N,
+                 int64_t E, int64_t L, int64_t D, int training, float momentum, float eps, const Drops& drops, int precision,
+                 float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes, void* stream) {
   PGNN_CHECK_ARG(valid_conv(conv_type) && N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && bn_running_mean && bn_running_var &&
                  workspace);
   PGNN_CHECK_ARG(N == 0 || (x && node_rep));
@@ -581,19 +556,20 @@ int pgnn_chem_conv_forward(int conv_type, const void* const* params, void* const
                        w.alpha + l * (E + N) * kHeads, w.pq + l * N * kHeads * 2, z, D, stream));
     } else if (conv_type == PGNN_CONV_GCN) {
       TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_GCN, w.dinv, w.S, 9, (const float*)p[G_ET1],
-                                      (const float*)p[G_ET2], 6, 0, z, D, st, nullptr));
+                                      (const float*)p[G_ET2], 6, 0, z, D, st, nullptr, nullptr));
     } else {
       // mean aggregation into the backward scratch `gz` (only its normalised rows and their norms are needed later)
       TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_MEAN, nullptr, w.S, 9, (const float*)p[G_ET1],
-                                      (const float*)p[G_ET2], 6, 0, w.gz, D, st, nullptr));
+                                      (const float*)p[G_ET2], 6, 0, w.gz, D, st, nullptr, nullptr));
       TRY(pgnn_l2norm_fwd(w.gz, D, N, D, z, D, w.nrm + l * N, stream));
     }
     const float* gamma = (const float*)p[gat ? A_GAMMA : G_GAMMA];
     const float* beta = (const float*)p[gat ? A_BETA : G_BETA];
     if (training) {
-      TRY(pgnn_bn_fwd_train(z, D, N, D, gamma, beta, (float*)bn_running_mean[l], (float*)bn_running_var[l],
-                            bn_num_batches_tracked ? (int64_t*)bn_num_batches_tracked[l] : nullptr, momentum, eps, !last, hout, ldh, w.mean + l * D,
-                            w.invstd + l * D, nullptr, nullptr, w.scratch, w.scratch_bytes, stream));
+      const PgnnDropout drop = drops.at(l);  // after the ReLU: hout is the next layer's input and its Linear's weight-gradient operand
+      TRY(pgnn_internal_bn_fwd_train(z, D, N, D, gamma, beta, (float*)bn_running_mean[l], (float*)bn_running_var[l],
+                                     bn_num_batches_tracked ? (int64_t*)bn_num_batches_tracked[l] : nullptr, momentum, eps, !last, hout, ldh,
+                                     w.mean + l * D, w.invstd + l * D, nullptr, nullptr, w.scratch, w.scratch_bytes, stream, &drop));
     } else {
       TRY(pgnn_bn_fwd_eval(z, D, N, D, gamma, beta, (const float*)bn_running_mean[l], (const float*)bn_running_var[l], eps, !last, hout, ldh, stream));
     }
@@ -602,9 +578,9 @@ int pgnn_chem_conv_forward(int conv_type, const void* const* params, void* const
   return PGNN_OK;
 }
 
-int pgnn_chem_conv_backward(int conv_type, const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x,
-                            const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, int precision, float* grads,
-                            void* workspace, int64_t workspace_bytes, void* stream) {
+int conv_backward(int conv_type, const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x,
+                  const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, const Drops& drops, int precision, float* grads,
+                  void* workspace, int64_t workspace_bytes, void* stream) {
   PGNN_CHECK_ARG(valid_conv(conv_type) && N >= 0 && E >= 0 && L >= 1 && L <= 64 && D > 0 && D % 4 == 0 && params && grads && workspace);
   if (workspace_bytes < pgnn_chem_conv_workspace_bytes(conv_type, N, E, L, D)) return PGNN_EWORKSPACE;
   int64_t off[2 + A_COUNT * 64 + 1];
@@ -634,8 +610,9 @@ int pgnn_chem_conv_backward(int conv_type, const void* const* params, const floa
     float* gxl = w.gxl + (sc ? par * N * HD : 0);
     const float* gamma = (const float*)p[gat ? A_GAMMA : G_GAMMA];
     const float* beta = (const float*)p[gat ? A_BETA : G_BETA];
-    TRY(pgnn_bn_bwd(gy, ldgy, z, D, N, D, gamma, beta, w.mean + l * D, w.invstd + l * D, !last, w.gz, D, grads + o[gat ? A_GAMMA : G_GAMMA],
-                    grads + o[gat ? A_BETA : G_BETA], w.scratch, w.scratch_bytes, stream));
+    const PgnnDropout drop = drops.at(l);
+    TRY(pgnn_internal_bn_bwd(gy, ldgy, z, D, N, D, gamma, beta, w.mean + l * D, w.invstd + l * D, !last, w.gz, D,
+                             grads + o[gat ? A_GAMMA : G_GAMMA], grads + o[gat ? A_BETA : G_BETA], w.scratch, w.scratch_bytes, stream, &drop));
     if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad has finished reading this copy of gxl
     if (gat) {
       // gT [9, HD] lands on the two adjacent bond-table gradients
@@ -672,6 +649,120 @@ int pgnn_chem_conv_backward(int conv_type, const void* const* params, const floa
     ldgy = D;
   }
   return embed_backward(sc, w, w.gh, x, N, D, precision, grads, off, w.wpart, w.wpart_floats, st);
+}
+
+}  // namespace
+
+extern "C" {
+
+// ------------------------------------------------------------------------------------------------------------------------------
+// GIN
+// ------------------------------------------------------------------------------------------------------------------------------
+int64_t pgnn_chem_gin_num_params(int64_t L) { return L < 1 ? PGNN_EINVAL : grad_layout(kGin, L, 0, nullptr); }
+
+int pgnn_chem_gin_grad_offsets(int64_t L, int64_t D, int64_t* offsets /*host [num_params + 1]*/) {
+  PGNN_CHECK_ARG(L >= 1 && D > 0 && offsets);
+  grad_layout(kGin, L, D, offsets);
+  return PGNN_OK;
+}
+
+int64_t pgnn_chem_gin_workspace_bytes(int64_t N, int64_t E, int64_t L, int64_t D) {
+  if (N < 0 || E < 0 || L < 1 || D <= 0) return PGNN_EINVAL;
+  return carve_gin(nullptr, N, E, L, D).total;
+}
+
+int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
+                          void* const* bn_num_batches_tracked, const int64_t* x, const int64_t* edge_index,
+                          const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, int training, float momentum, float eps,
+                          int precision, float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes, void* stream) {
+  return pgnn_chem_encoder_forward(kGin, params, bn_running_mean, bn_running_var, bn_num_batches_tracked, x, edge_index, edge_attr, N, E, L, D,
+                                   training, momentum, eps, 0.f, 0, precision, node_rep, ld_out, workspace, workspace_bytes, stream);
+}
+
+int pgnn_chem_gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x, int64_t N, int64_t E,
+                           int64_t L, int64_t D, int precision, float* grads, void* workspace, int64_t workspace_bytes,
+                           void* stream) {
+  return pgnn_chem_encoder_backward(kGin, params, g_node_rep, ldg, x, nullptr, N, E, L, D, 0.f, 0, precision, grads, workspace,
+                                    workspace_bytes, stream);
+}
+
+// Development / test aid: byte offsets inside the workspace of the saved activations a test needs to reconstruct the
+// ReLU decisions the encoder actually took: out[0] = z1 (post-ReLU hidden activations, [L][N][2D]), out[1] = z2 (pre-BatchNorm
+// layer outputs, [L][N][D]), out[2] = BatchNorm batch mean [L][D], out[3] = invstd [L][D].
+int pgnn_chem_gin_debug_layout(int64_t N, int64_t E, int64_t L, int64_t D, int64_t* out4) {
+  PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && out4);
+  char* base = reinterpret_cast<char*>(0x1000);  // carve_gin() only does pointer arithmetic
+  GinWs w = carve_gin(base, N, E, L, D);
+  out4[0] = reinterpret_cast<char*>(w.z1) - base;
+  out4[1] = reinterpret_cast<char*>(w.z2) - base;
+  out4[2] = reinterpret_cast<char*>(w.mean) - base;
+  out4[3] = reinterpret_cast<char*>(w.invstd) - base;
+  return PGNN_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------------------------
+// GCN / GraphSAGE / GAT
+// ------------------------------------------------------------------------------------------------------------------------------
+int64_t pgnn_chem_conv_num_params(int conv_type, int64_t L) {
+  if (!valid_conv(conv_type) || L < 1) return PGNN_EINVAL;
+  return grad_layout(conv_type, L, 0, nullptr);
+}
+
+int pgnn_chem_conv_grad_offsets(int conv_type, int64_t L, int64_t D, int64_t* offsets) {
+  PGNN_CHECK_ARG(valid_conv(conv_type) && L >= 1 && D > 0 && offsets);
+  grad_layout(conv_type, L, D, offsets);
+  return PGNN_OK;
+}
+
+int64_t pgnn_chem_conv_workspace_bytes(int conv_type, int64_t N, int64_t E, int64_t L, int64_t D) {
+  if (!valid_conv(conv_type) || N < 0 || E < 0 || L < 1 || D <= 0) return PGNN_EINVAL;
+  return carve_conv(nullptr, conv_type, N, E, L, D).total;
+}
+
+int pgnn_chem_conv_forward(int conv_type, const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
+                           void* const* bn_num_batches_tracked, const int64_t* x, const int64_t* edge_index, const int64_t* edge_attr,
+                           int64_t N, int64_t E, int64_t L, int64_t D, int training, float momentum, float eps, int precision,
+                           float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes, void* stream) {
+  PGNN_CHECK_ARG(valid_conv(conv_type));
+  return pgnn_chem_encoder_forward(conv_type, params, bn_running_mean, bn_running_var, bn_num_batches_tracked, x, edge_index, edge_attr, N, E, L,
+                                   D, training, momentum, eps, 0.f, 0, precision, node_rep, ld_out, workspace, workspace_bytes, stream);
+}
+
+int pgnn_chem_conv_backward(int conv_type, const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x,
+                            const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, int precision, float* grads,
+                            void* workspace, int64_t workspace_bytes, void* stream) {
+  PGNN_CHECK_ARG(valid_conv(conv_type));
+  return pgnn_chem_encoder_backward(conv_type, params, g_node_rep, ldg, x, edge_attr, N, E, L, D, 0.f, 0, precision, grads, workspace,
+                                    workspace_bytes, stream);
+}
+
+// ------------------------------------------------------------------------------------------------------------------------------
+// every type, with dropout
+// ------------------------------------------------------------------------------------------------------------------------------
+int pgnn_chem_encoder_forward(int gnn_type, const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
+                              void* const* bn_num_batches_tracked, const int64_t* x, const int64_t* edge_index, const int64_t* edge_attr,
+                              int64_t N, int64_t E, int64_t L, int64_t D, int training, float momentum, float eps, float drop_p,
+                              int64_t drop_seed, int precision, float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes,
+                              void* stream) {
+  PGNN_CHECK_ARG((gnn_type == kGin || valid_conv(gnn_type)) && drop_p >= 0.f && drop_p <= 1.f);
+  Drops drops;
+  if (training) drops = Drops{drop_p, drop_seed};  // eval mode has no dropout
+  if (gnn_type == kGin)
+    return gin_forward(params, bn_running_mean, bn_running_var, bn_num_batches_tracked, x, edge_index, edge_attr, N, E, L, D, training, momentum,
+                       eps, drops, precision, node_rep, ld_out, workspace, workspace_bytes, stream);
+  return conv_forward(gnn_type, params, bn_running_mean, bn_running_var, bn_num_batches_tracked, x, edge_index, edge_attr, N, E, L, D, training,
+                      momentum, eps, drops, precision, node_rep, ld_out, workspace, workspace_bytes, stream);
+}
+
+int pgnn_chem_encoder_backward(int gnn_type, const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x,
+                               const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, float drop_p, int64_t drop_seed,
+                               int precision, float* grads, void* workspace, int64_t workspace_bytes, void* stream) {
+  PGNN_CHECK_ARG((gnn_type == kGin || valid_conv(gnn_type)) && drop_p >= 0.f && drop_p <= 1.f);
+  const Drops drops{drop_p, drop_seed};
+  if (gnn_type == kGin)
+    return gin_backward(params, g_node_rep, ldg, x, N, E, L, D, drops, precision, grads, workspace, workspace_bytes, stream);
+  return conv_backward(gnn_type, params, g_node_rep, ldg, x, edge_attr, N, E, L, D, drops, precision, grads, workspace, workspace_bytes,
+                       stream);
 }
 
 }  // extern "C"

@@ -28,13 +28,6 @@ constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 enum { Q_NS = 0, Q_ES, Q_NC, Q_EC, Q_KO, Q_KEPT, Q_COUNT };
 
-__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t seed, uint64_t idx) {
-  uint64_t z = seed + (idx + 1ull) * 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
 struct Ws {
   int64_t *full_node_off, *counts;  // [B+1], [Q_COUNT][B]
   int32_t *root, *dist, *map_s, *map_c;  // [B], [Nfull] x 3

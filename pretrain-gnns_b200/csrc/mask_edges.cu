@@ -21,13 +21,6 @@ constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 constexpr int kKeyCache = 4096;  // pairs whose keys fit the CTA's shared memory (32 KB); larger graphs recompute keys
 
-__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t seed, uint64_t idx) {
-  uint64_t z = seed + (idx + 1ull) * 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
 __device__ __forceinline__ int64_t edge_mask_count(int64_t pairs, double rate) {
   if (pairs <= 0) return 0;
   const int64_t k = (int64_t)((double)pairs * rate + 1.0);  // int(num_edges * mask_rate + 1), bio/util.py:80

@@ -91,10 +91,14 @@ k_bn_finalize(const double* __restrict__ acc, int M, int C, const float* __restr
   }
 }
 
-__global__ void __launch_bounds__(256)
-k_bn_apply(const float* __restrict__ x, int64_t ldx, int64_t M, int C, const float* __restrict__ mean,
-           const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
-           float* __restrict__ y, int64_t ldy) {
+// Kernels that may carry dropout are written once as a `template <bool DROP>` body: the DROP = false instantiation is the
+// kernel of the same name (no mask), DROP = true the `_drop` kernel, which multiplies by the mask of PgnnDropout `drop`
+// (forward: after the ReLU; backward: the incoming gradient, before the ReLU mask).
+template <bool DROP>
+__device__ __forceinline__ void bn_apply_body(const float* __restrict__ x, int64_t ldx, int64_t M, int C, const float* __restrict__ mean,
+                                              const float* __restrict__ invstd, const float* __restrict__ gamma,
+                                              const float* __restrict__ beta, int relu, float* __restrict__ y, int64_t ldy,
+                                              const PgnnDropout& drop) {
   pdl_prologue();
   const int64_t total = M * C;
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
@@ -102,14 +106,27 @@ k_bn_apply(const float* __restrict__ x, int64_t ldx, int64_t M, int C, const flo
     const int c = (int)(idx - r * C);
     float v = fmaf((x[r * ldx + c] - mean[c]) * invstd[c], gamma[c], beta[c]);
     if (relu) v = relu_keep_nan(v);
+    if (DROP) v *= dropout_factor(drop, r, C, c);
     y[r * ldy + c] = v;
   }
 }
+__global__ void __launch_bounds__(256)
+k_bn_apply(const float* __restrict__ x, int64_t ldx, int64_t M, int C, const float* __restrict__ mean,
+           const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
+           float* __restrict__ y, int64_t ldy) {
+  bn_apply_body<false>(x, ldx, M, C, mean, invstd, gamma, beta, relu, y, ldy, PgnnDropout{});
+}
+__global__ void __launch_bounds__(256)
+k_bn_apply_drop(const float* __restrict__ x, int64_t ldx, int64_t M, int C, const float* __restrict__ mean,
+                const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
+                float* __restrict__ y, int64_t ldy, PgnnDropout drop) {
+  bn_apply_body<true>(x, ldx, M, C, mean, invstd, gamma, beta, relu, y, ldy, drop);
+}
 
 // BatchNorm apply with the finalisation folded in (the last encoder layer materialises node_rep this way)
-__global__ void __launch_bounds__(256)
-k_bn_apply_fold(const float* __restrict__ x, int64_t ldx, int64_t M, int C, PgnnBnFold fold, int relu, float* __restrict__ y,
-                int64_t ldy) {
+template <bool DROP>
+__device__ __forceinline__ void bn_apply_fold_body(const float* __restrict__ x, int64_t ldx, int64_t M, int C, const PgnnBnFold& fold,
+                                                   int relu, float* __restrict__ y, int64_t ldy, const PgnnDropout& drop) {
   pdl_prologue();
   extern __shared__ __align__(16) float s_aff[];
   for (int c = threadIdx.x; c < C; c += blockDim.x) bn_fold_column(fold, C, c, blockIdx.x == 0, s_aff[c], s_aff[C + c]);
@@ -120,8 +137,19 @@ k_bn_apply_fold(const float* __restrict__ x, int64_t ldx, int64_t M, int C, Pgnn
     const int c = (int)(idx - r * C);
     float v = fmaf(x[r * ldx + c], s_aff[c], s_aff[C + c]);
     if (relu) v = relu_keep_nan(v);
+    if (DROP) v *= dropout_factor(drop, r, C, c);
     y[r * ldy + c] = v;
   }
+}
+__global__ void __launch_bounds__(256)
+k_bn_apply_fold(const float* __restrict__ x, int64_t ldx, int64_t M, int C, PgnnBnFold fold, int relu, float* __restrict__ y,
+                int64_t ldy) {
+  bn_apply_fold_body<false>(x, ldx, M, C, fold, relu, y, ldy, PgnnDropout{});
+}
+__global__ void __launch_bounds__(256)
+k_bn_apply_fold_drop(const float* __restrict__ x, int64_t ldx, int64_t M, int C, PgnnBnFold fold, int relu, float* __restrict__ y,
+                     int64_t ldy, PgnnDropout drop) {
+  bn_apply_fold_body<true>(x, ldx, M, C, fold, relu, y, ldy, drop);
 }
 
 __global__ void __launch_bounds__(256)
@@ -140,18 +168,32 @@ k_bn_eval(const float* __restrict__ x, int64_t ldx, int64_t M, int C, const floa
   }
 }
 
-__global__ void __launch_bounds__(256)
-k_bn_bwd_stats(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
-               const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
-               const float* __restrict__ invstd, int relu, double* __restrict__ acc) {
+template <bool DROP>
+__device__ __forceinline__ void bn_bwd_stats_body(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx,
+                                                  int M, int C, const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                  const float* __restrict__ mean, const float* __restrict__ invstd, int relu,
+                                                  double* __restrict__ acc, const PgnnDropout& drop) {
   pdl_prologue();
   column_pair_sums(M, C, acc, [&](int r, int c, double& a, double& b) {
     const float xhat = (x[(int64_t)r * ldx + c] - mean[c]) * invstd[c];
     float d = gy[(int64_t)r * ldgy + c];
+    if (DROP) d *= dropout_factor(drop, r, C, c);
     if (relu && !(fmaf(xhat, gamma[c], beta[c]) > 0.f)) d = 0.f;
     a = (double)d;
     b = (double)d * (double)xhat;  // exact product: small batches make the BN backward a difference of large terms
   });
+}
+__global__ void __launch_bounds__(256)
+k_bn_bwd_stats(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
+               const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
+               const float* __restrict__ invstd, int relu, double* __restrict__ acc) {
+  bn_bwd_stats_body<false>(gy, ldgy, x, ldx, M, C, gamma, beta, mean, invstd, relu, acc, PgnnDropout{});
+}
+__global__ void __launch_bounds__(256)
+k_bn_bwd_stats_drop(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
+                    const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
+                    const float* __restrict__ invstd, int relu, double* __restrict__ acc, PgnnDropout drop) {
+  bn_bwd_stats_body<true>(gy, ldgy, x, ldx, M, C, gamma, beta, mean, invstd, relu, acc, drop);
 }
 
 __global__ void __launch_bounds__(128)
@@ -167,11 +209,12 @@ k_bn_bwd_finalize(const double* __restrict__ acc, int M, int C, float* __restric
   c2[c] = (float)(sx / M);
 }
 
-__global__ void __launch_bounds__(256)
-k_bn_bwd_apply(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int64_t M, int C,
-               const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
-               const float* __restrict__ invstd, int relu, const float* __restrict__ c1, const float* __restrict__ c2,
-               float* __restrict__ gx, int64_t ldgx) {
+template <bool DROP>
+__device__ __forceinline__ void bn_bwd_apply_body(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx,
+                                                  int64_t M, int C, const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                  const float* __restrict__ mean, const float* __restrict__ invstd, int relu,
+                                                  const float* __restrict__ c1, const float* __restrict__ c2, float* __restrict__ gx,
+                                                  int64_t ldgx, const PgnnDropout& drop) {
   pdl_prologue();
   const int64_t total = M * C;
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
@@ -179,18 +222,35 @@ k_bn_bwd_apply(const float* __restrict__ gy, int64_t ldgy, const float* __restri
     const int c = (int)(idx - r * C);
     const float xhat = (x[r * ldx + c] - mean[c]) * invstd[c];
     float d = gy[r * ldgy + c];
+    if (DROP) d *= dropout_factor(drop, r, C, c);
     if (relu && !(fmaf(xhat, gamma[c], beta[c]) > 0.f)) d = 0.f;
     gx[r * ldgx + c] = gamma[c] * invstd[c] * (d - c1[c] - xhat * c2[c]);
   }
 }
+__global__ void __launch_bounds__(256)
+k_bn_bwd_apply(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int64_t M, int C,
+               const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
+               const float* __restrict__ invstd, int relu, const float* __restrict__ c1, const float* __restrict__ c2,
+               float* __restrict__ gx, int64_t ldgx) {
+  bn_bwd_apply_body<false>(gy, ldgy, x, ldx, M, C, gamma, beta, mean, invstd, relu, c1, c2, gx, ldgx, PgnnDropout{});
+}
+__global__ void __launch_bounds__(256)
+k_bn_bwd_apply_drop(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int64_t M, int C,
+                    const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
+                    const float* __restrict__ invstd, int relu, const float* __restrict__ c1, const float* __restrict__ c2,
+                    float* __restrict__ gx, int64_t ldgx, PgnnDropout drop) {
+  bn_bwd_apply_body<true>(gy, ldgy, x, ldx, M, C, gamma, beta, mean, invstd, relu, c1, c2, gx, ldgx, drop);
+}
 
 // same arithmetic as k_bn_bwd_apply in the 32-column x 8-row-lane block shape of the statistics sweeps, so that the
 // column sums of gx (= the bias gradient of the Linear that produced x, chem/model.py:29 mlp[2]) fall out of the same pass
-__global__ void __launch_bounds__(256)
-k_bn_bwd_apply_colsum(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
-                      const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
-                      const float* __restrict__ invstd, int relu, const double* __restrict__ sums, float* __restrict__ ggamma,
-                      float* __restrict__ gbeta, float* __restrict__ gx, int64_t ldgx, float* __restrict__ colsum) {
+template <bool DROP>
+__device__ __forceinline__ void bn_bwd_apply_colsum_body(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x,
+                                                         int64_t ldx, int M, int C, const float* __restrict__ gamma,
+                                                         const float* __restrict__ beta, const float* __restrict__ mean,
+                                                         const float* __restrict__ invstd, int relu, const double* __restrict__ sums,
+                                                         float* __restrict__ ggamma, float* __restrict__ gbeta, float* __restrict__ gx,
+                                                         int64_t ldgx, float* __restrict__ colsum, const PgnnDropout& drop) {
   pdl_prologue();
   __shared__ float red[8][33];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -209,6 +269,7 @@ k_bn_bwd_apply_colsum(const float* __restrict__ gy, int64_t ldgy, const float* _
     for (int r = r0 + w; r < r1; r += 8) {
       const float xhat = (x[(int64_t)r * ldx + c] - mu) * is;
       float d = gy[(int64_t)r * ldgy + c];
+      if (DROP) d *= dropout_factor(drop, r, C, c);
       if (relu && !(fmaf(xhat, ga, be) > 0.f)) d = 0.f;
       const float v = ga * is * (d - k1 - xhat * k2);
       gx[(int64_t)r * ldgx + c] = v;
@@ -224,6 +285,22 @@ k_bn_bwd_apply_colsum(const float* __restrict__ gy, int64_t ldgy, const float* _
     atomicAdd(&colsum[c], t);
   }
 }
+__global__ void __launch_bounds__(256)
+k_bn_bwd_apply_colsum(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
+                      const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
+                      const float* __restrict__ invstd, int relu, const double* __restrict__ sums, float* __restrict__ ggamma,
+                      float* __restrict__ gbeta, float* __restrict__ gx, int64_t ldgx, float* __restrict__ colsum) {
+  bn_bwd_apply_colsum_body<false>(gy, ldgy, x, ldx, M, C, gamma, beta, mean, invstd, relu, sums, ggamma, gbeta, gx, ldgx, colsum,
+                                  PgnnDropout{});
+}
+__global__ void __launch_bounds__(256)
+k_bn_bwd_apply_colsum_drop(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
+                           const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
+                           const float* __restrict__ invstd, int relu, const double* __restrict__ sums, float* __restrict__ ggamma,
+                           float* __restrict__ gbeta, float* __restrict__ gx, int64_t ldgx, float* __restrict__ colsum,
+                           PgnnDropout drop) {
+  bn_bwd_apply_colsum_body<true>(gy, ldgy, x, ldx, M, C, gamma, beta, mean, invstd, relu, sums, ggamma, gbeta, gx, ldgx, colsum, drop);
+}
 
 // ---- 16-byte versions of the two BatchNorm-backward sweeps (encoder path: C % 4 == 0, aligned rows) ----------------------
 // Tile = 128 columns (one float4 per lane) x kVecRows rows; warp w walks rows r0 + w, r0 + w + 8, ...: every load is a
@@ -232,10 +309,12 @@ constexpr int kVecRows = 64;
 
 __device__ __forceinline__ float4 ldg4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
-__global__ void __launch_bounds__(256)
-k_bn_bwd_stats_v4(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
-                  const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
-                  const float* __restrict__ invstd, int relu, double* __restrict__ acc) {
+template <bool DROP>
+__device__ __forceinline__ void bn_bwd_stats_v4_body(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x,
+                                                     int64_t ldx, int M, int C, const float* __restrict__ gamma,
+                                                     const float* __restrict__ beta, const float* __restrict__ mean,
+                                                     const float* __restrict__ invstd, int relu, double* __restrict__ acc,
+                                                     const PgnnDropout& drop) {
   pdl_prologue();
   __shared__ double red[2][8][128];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -254,6 +333,7 @@ k_bn_bwd_stats_v4(const float* __restrict__ gy, int64_t ldgy, const float* __res
       for (int q = 0; q < 4; ++q) {
         const float xhat = (xs[q] - muv[q]) * isv[q];
         float d = gs[q];
+        if (DROP) d *= dropout_factor(drop, r, C, c + q);
         if (relu && !(fmaf(xhat, gav[q], bev[q]) > 0.f)) d = 0.f;
         s0[q] += (double)d;
         s1[q] += (double)d * (double)xhat;
@@ -274,12 +354,27 @@ k_bn_bwd_stats_v4(const float* __restrict__ gy, int64_t ldgy, const float* __res
     atomicAdd(&acc[(int64_t)which * C + blockIdx.x * 128 + col], t);
   }
 }
-
 __global__ void __launch_bounds__(256)
-k_bn_bwd_apply_colsum_v4(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
-                         const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
-                         const float* __restrict__ invstd, int relu, const double* __restrict__ sums, float* __restrict__ ggamma,
-                         float* __restrict__ gbeta, float* __restrict__ gx, int64_t ldgx, float* __restrict__ colsum) {
+k_bn_bwd_stats_v4(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
+                  const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
+                  const float* __restrict__ invstd, int relu, double* __restrict__ acc) {
+  bn_bwd_stats_v4_body<false>(gy, ldgy, x, ldx, M, C, gamma, beta, mean, invstd, relu, acc, PgnnDropout{});
+}
+__global__ void __launch_bounds__(256)
+k_bn_bwd_stats_v4_drop(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
+                       const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
+                       const float* __restrict__ invstd, int relu, double* __restrict__ acc, PgnnDropout drop) {
+  bn_bwd_stats_v4_body<true>(gy, ldgy, x, ldx, M, C, gamma, beta, mean, invstd, relu, acc, drop);
+}
+
+template <bool DROP>
+__device__ __forceinline__ void bn_bwd_apply_colsum_v4_body(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x,
+                                                            int64_t ldx, int M, int C, const float* __restrict__ gamma,
+                                                            const float* __restrict__ beta, const float* __restrict__ mean,
+                                                            const float* __restrict__ invstd, int relu,
+                                                            const double* __restrict__ sums, float* __restrict__ ggamma,
+                                                            float* __restrict__ gbeta, float* __restrict__ gx, int64_t ldgx,
+                                                            float* __restrict__ colsum, const PgnnDropout& drop) {
   pdl_prologue();
   __shared__ float red[8][128];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -310,6 +405,7 @@ k_bn_bwd_apply_colsum_v4(const float* __restrict__ gy, int64_t ldgy, const float
       for (int q = 0; q < 4; ++q) {
         const float xhat = (xs[q] - muv[q]) * isv[q];
         float d = gs[q];
+        if (DROP) d *= dropout_factor(drop, r, C, c + q);
         if (relu && !(fmaf(xhat, gav[q], bev[q]) > 0.f)) d = 0.f;
         o[q] = gav[q] * isv[q] * (d - k1[q] - xhat * k2[q]);
         acc[q] += o[q];
@@ -326,6 +422,23 @@ k_bn_bwd_apply_colsum_v4(const float* __restrict__ gy, int64_t ldgy, const float
     for (int k = 0; k < 8; ++k) t += red[k][threadIdx.x];
     atomicAdd(&colsum[blockIdx.x * 128 + threadIdx.x], t);
   }
+}
+__global__ void __launch_bounds__(256)
+k_bn_bwd_apply_colsum_v4(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
+                         const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
+                         const float* __restrict__ invstd, int relu, const double* __restrict__ sums, float* __restrict__ ggamma,
+                         float* __restrict__ gbeta, float* __restrict__ gx, int64_t ldgx, float* __restrict__ colsum) {
+  bn_bwd_apply_colsum_v4_body<false>(gy, ldgy, x, ldx, M, C, gamma, beta, mean, invstd, relu, sums, ggamma, gbeta, gx, ldgx, colsum,
+                                     PgnnDropout{});
+}
+__global__ void __launch_bounds__(256)
+k_bn_bwd_apply_colsum_v4_drop(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
+                              const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
+                              const float* __restrict__ invstd, int relu, const double* __restrict__ sums,
+                              float* __restrict__ ggamma, float* __restrict__ gbeta, float* __restrict__ gx, int64_t ldgx,
+                              float* __restrict__ colsum, PgnnDropout drop) {
+  bn_bwd_apply_colsum_v4_body<true>(gy, ldgy, x, ldx, M, C, gamma, beta, mean, invstd, relu, sums, ggamma, gbeta, gx, ldgx, colsum,
+                                    drop);
 }
 
 // forward statistics and apply in the same 16-byte tiling
@@ -364,10 +477,11 @@ k_bn_stats_v4(const float* __restrict__ x, int64_t ldx, int M, int C, double* __
   }
 }
 
-__global__ void __launch_bounds__(256)
-k_bn_apply_v4(const float* __restrict__ x, int64_t ldx, int64_t M, int C4, const float* __restrict__ mean,
-              const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
-              float* __restrict__ y, int64_t ldy) {
+template <bool DROP>
+__device__ __forceinline__ void bn_apply_v4_body(const float* __restrict__ x, int64_t ldx, int64_t M, int C4,
+                                                 const float* __restrict__ mean, const float* __restrict__ invstd,
+                                                 const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
+                                                 float* __restrict__ y, int64_t ldy, const PgnnDropout& drop) {
   pdl_prologue();
   const int64_t total = M * C4;
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
@@ -382,8 +496,21 @@ k_bn_apply_v4(const float* __restrict__ x, int64_t ldx, int64_t M, int C4, const
     if (relu) {
       o.x = relu_keep_nan(o.x); o.y = relu_keep_nan(o.y); o.z = relu_keep_nan(o.z); o.w = relu_keep_nan(o.w);
     }
+    if (DROP) o = dropout4(o, drop, r, 4 * (int64_t)C4, c);
     *reinterpret_cast<float4*>(y + r * ldy + c) = o;
   }
+}
+__global__ void __launch_bounds__(256)
+k_bn_apply_v4(const float* __restrict__ x, int64_t ldx, int64_t M, int C4, const float* __restrict__ mean,
+              const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
+              float* __restrict__ y, int64_t ldy) {
+  bn_apply_v4_body<false>(x, ldx, M, C4, mean, invstd, gamma, beta, relu, y, ldy, PgnnDropout{});
+}
+__global__ void __launch_bounds__(256)
+k_bn_apply_v4_drop(const float* __restrict__ x, int64_t ldx, int64_t M, int C4, const float* __restrict__ mean,
+                   const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
+                   float* __restrict__ y, int64_t ldy, PgnnDropout drop) {
+  bn_apply_v4_body<true>(x, ldx, M, C4, mean, invstd, gamma, beta, relu, y, ldy, drop);
 }
 
 __global__ void __launch_bounds__(256)
@@ -477,21 +604,32 @@ inline int grid_items(int64_t items, int threads) {
   return (int)(b < 1 ? 1 : b);
 }
 
+// the dropout a caller asked for, or null when there is none (p == 0 is inert: the kernels without a mask run)
+inline const PgnnDropout* live(const PgnnDropout* d) { return d && d->p > 0.f ? d : nullptr; }
+
 }  // namespace
 
 // encoder.cu: BatchNorm forward when the column sums / sums of squares were already accumulated (fp64, [2][C]) by the
 // epilogue of the GEMM that produced x (PgnnGemmHooks::stats)
+// (drop: the mask applied after the ReLU, or null)
 int pgnn_internal_bn_apply_fold(const float* x, int64_t ldx, int64_t M, int64_t C, const PgnnBnFold& fold, int relu, float* y,
-                                int64_t ldy, cudaStream_t st) {
-  PGNN_CUDA(pgnn_launch(k_bn_apply_fold, dim3(grid_items(M * C, 256)), dim3(256), sizeof(float) * 2 * C, st, x, ldx, M, (int)C, fold, relu, y, ldy));
+                                int64_t ldy, cudaStream_t st, const PgnnDropout* drop) {
+  const dim3 grid(grid_items(M * C, 256));
+  if (const PgnnDropout* d = live(drop))
+    PGNN_CUDA(pgnn_launch(k_bn_apply_fold_drop, grid, dim3(256), sizeof(float) * 2 * C, st, x, ldx, M, (int)C, fold, relu, y, ldy, *d));
+  else
+    PGNN_CUDA(pgnn_launch(k_bn_apply_fold, grid, dim3(256), sizeof(float) * 2 * C, st, x, ldx, M, (int)C, fold, relu, y, ldy));
   PGNN_LAUNCH_CHECK();
   return PGNN_OK;
 }
 
-// encoder.cu: pgnn_bn_bwd that also leaves the column sums of gx in colsum[C] (OVERWRITTEN)
+// encoder.cu: pgnn_bn_bwd that also leaves the column sums of gx in colsum[C] (OVERWRITTEN).  drop: the forward's mask, applied
+// to gy before the ReLU mask, or null.
 int pgnn_internal_bn_bwd_colsum(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma,
                                 const float* beta, const float* save_mean, const float* save_invstd, int relu, float* gx,
-                                int64_t ldgx, float* ggamma, float* gbeta, float* colsum, void* workspace, cudaStream_t st) {
+                                int64_t ldgx, float* ggamma, float* gbeta, float* colsum, void* workspace, cudaStream_t st,
+                                const PgnnDropout* drop) {
+  const PgnnDropout* dr = live(drop);
   double* acc = reinterpret_cast<double*>(workspace);
   float* c1 = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + align_up(2 * C * 8, 256));
   float* c2 = c1 + C;
@@ -501,33 +639,44 @@ int pgnn_internal_bn_bwd_colsum(const float* gy, int64_t ldgy, const float* x, i
   if (bn_v4_enabled() && C % 4 == 0 && ldgy % 4 == 0 && ldx % 4 == 0 && ldgx % 4 == 0 && a16(gy) && a16(x) && a16(gx) && a16(gamma) && a16(beta) &&
       a16(save_mean) && a16(save_invstd)) {
     dim3 gv((unsigned)ceil_div(C, 128), (unsigned)ceil_div(M, kVecRows));
-    PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_v4, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu, acc));
+    if (dr)
+      PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_v4_drop, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd,
+                            relu, acc, *dr));
+    else
+      PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_v4, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu, acc));
     PGNN_LAUNCH_CHECK();
-    PGNN_CUDA(pgnn_launch(k_bn_bwd_apply_colsum_v4, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd,
-                          relu, (const double*)acc, ggamma, gbeta, gx, ldgx, colsum));
+    if (dr)
+      PGNN_CUDA(pgnn_launch(k_bn_bwd_apply_colsum_v4_drop, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean,
+                            save_invstd, relu, (const double*)acc, ggamma, gbeta, gx, ldgx, colsum, *dr));
+    else
+      PGNN_CUDA(pgnn_launch(k_bn_bwd_apply_colsum_v4, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd,
+                            relu, (const double*)acc, ggamma, gbeta, gx, ldgx, colsum));
     PGNN_LAUNCH_CHECK();
     return PGNN_OK;
   }
   dim3 g1((unsigned)ceil_div(C, 32), (unsigned)ceil_div(M, kStatRows));
-  PGNN_CUDA(pgnn_launch(k_bn_bwd_stats, dim3(g1), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu, acc));
+  if (dr)
+    PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_drop, dim3(g1), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu,
+                          acc, *dr));
+  else
+    PGNN_CUDA(pgnn_launch(k_bn_bwd_stats, dim3(g1), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu, acc));
   PGNN_LAUNCH_CHECK();
-  PGNN_CUDA(pgnn_launch(k_bn_bwd_apply_colsum, dim3(g1), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu,
-                        (const double*)acc, ggamma, gbeta, gx, ldgx, colsum));
+  if (dr)
+    PGNN_CUDA(pgnn_launch(k_bn_bwd_apply_colsum_drop, dim3(g1), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd,
+                          relu, (const double*)acc, ggamma, gbeta, gx, ldgx, colsum, *dr));
+  else
+    PGNN_CUDA(pgnn_launch(k_bn_bwd_apply_colsum, dim3(g1), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu,
+                          (const double*)acc, ggamma, gbeta, gx, ldgx, colsum));
   PGNN_LAUNCH_CHECK();
   return PGNN_OK;
 }
 
-extern "C" {
-
-int64_t pgnn_bn_workspace_bytes(int64_t M, int64_t C) {
-  if (M < 0 || C <= 0) return PGNN_EINVAL;
-  return align_up(2 * C * 8, 256) + align_up(2 * C * 4, 256);
-}
-
-int pgnn_bn_fwd_train(const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma, const float* beta,
-                      float* running_mean, float* running_var, int64_t* num_batches_tracked, float momentum, float eps, int relu,
-                      float* y, int64_t ldy, float* save_mean, float* save_invstd, float* scale, float* shift, void* workspace,
-                      int64_t workspace_bytes, void* stream) {
+// pgnn_bn_fwd_train with the mask `drop` (or null) applied after the ReLU of the materialised y (encoder.cu)
+int pgnn_internal_bn_fwd_train(const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma, const float* beta,
+                               float* running_mean, float* running_var, int64_t* num_batches_tracked, float momentum, float eps,
+                               int relu, float* y, int64_t ldy, float* save_mean, float* save_invstd, float* scale, float* shift,
+                               void* workspace, int64_t workspace_bytes, void* stream, const PgnnDropout* drop) {
+  const PgnnDropout* dr = live(drop);
   PGNN_CHECK_ARG(M > 0 && C > 0 && M < (1ll << 31) && x && gamma && beta && save_mean && save_invstd && workspace);
   PGNN_CHECK_ARG((scale == nullptr) == (shift == nullptr));
   if (workspace_bytes < pgnn_bn_workspace_bytes(M, C)) return PGNN_EWORKSPACE;
@@ -550,11 +699,84 @@ int pgnn_bn_fwd_train(const float* x, int64_t ldx, int64_t M, int64_t C, const f
                                                            shift));
   PGNN_LAUNCH_CHECK();
   if (y) {
-    if (v4) PGNN_CUDA(pgnn_launch(k_bn_apply_v4, dim3(grid_items(M * (C / 4), 256)), dim3(256), 0, st, x, ldx, M, (int)(C / 4), save_mean, save_invstd, gamma, beta, relu, y, ldy));
+    if (v4 && dr)
+      PGNN_CUDA(pgnn_launch(k_bn_apply_v4_drop, dim3(grid_items(M * (C / 4), 256)), dim3(256), 0, st, x, ldx, M, (int)(C / 4), save_mean, save_invstd, gamma,
+                            beta, relu, y, ldy, *dr));
+    else if (v4) PGNN_CUDA(pgnn_launch(k_bn_apply_v4, dim3(grid_items(M * (C / 4), 256)), dim3(256), 0, st, x, ldx, M, (int)(C / 4), save_mean, save_invstd, gamma, beta, relu, y, ldy));
+    else if (dr)
+      PGNN_CUDA(pgnn_launch(k_bn_apply_drop, dim3(grid_items(M * C, 256)), dim3(256), 0, st, x, ldx, M, (int)C, save_mean, save_invstd, gamma, beta, relu,
+                            y, ldy, *dr));
     else PGNN_CUDA(pgnn_launch(k_bn_apply, dim3(grid_items(M * C, 256)), dim3(256), 0, st, x, ldx, M, (int)C, save_mean, save_invstd, gamma, beta, relu, y, ldy));
     PGNN_LAUNCH_CHECK();
   }
   return PGNN_OK;
+}
+
+// pgnn_bn_bwd with the forward's mask `drop` (or null) applied to gy before the ReLU mask (encoder.cu)
+int pgnn_internal_bn_bwd(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma,
+                         const float* beta, const float* save_mean, const float* save_invstd, int relu, float* gx, int64_t ldgx,
+                         float* ggamma, float* gbeta, void* workspace, int64_t workspace_bytes, void* stream, const PgnnDropout* drop) {
+  const PgnnDropout* dr = live(drop);
+  PGNN_CHECK_ARG(M > 0 && C > 0 && M < (1ll << 31) && gy && x && gamma && beta && save_mean && save_invstd && gx && workspace);
+  if (workspace_bytes < pgnn_bn_workspace_bytes(M, C)) return PGNN_EWORKSPACE;
+  cudaStream_t st = as_stream(stream);
+  double* acc = reinterpret_cast<double*>(workspace);
+  float* c1 = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + align_up(2 * C * 8, 256));
+  float* c2 = c1 + C;
+  PGNN_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * 2 * C, st));
+  {
+    auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+    if (bn_v4_enabled() && C % 4 == 0 && ldgy % 4 == 0 && ldx % 4 == 0 && ldgx % 4 == 0 && a16(gy) && a16(x) && a16(gx) && a16(gamma) && a16(beta) &&
+        a16(save_mean) && a16(save_invstd)) {
+      dim3 gv((unsigned)ceil_div(C, 128), (unsigned)ceil_div(M, kVecRows));
+      if (dr)
+        PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_v4_drop, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd,
+                              relu, acc, *dr));
+      else
+        PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_v4, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu, acc));
+      PGNN_LAUNCH_CHECK();
+      if (dr)
+        PGNN_CUDA(pgnn_launch(k_bn_bwd_apply_colsum_v4_drop, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean,
+                              save_invstd, relu, (const double*)acc, ggamma, gbeta, gx, ldgx, (float*)nullptr, *dr));
+      else
+        PGNN_CUDA(pgnn_launch(k_bn_bwd_apply_colsum_v4, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd,
+                              relu, (const double*)acc, ggamma, gbeta, gx, ldgx, (float*)nullptr));
+      PGNN_LAUNCH_CHECK();
+      return PGNN_OK;
+    }
+  }
+  dim3 g1((unsigned)ceil_div(C, 32), (unsigned)ceil_div(M, kStatRows));
+  if (dr)
+    PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_drop, dim3(g1), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu,
+                          acc, *dr));
+  else
+    PGNN_CUDA(pgnn_launch(k_bn_bwd_stats, dim3(g1), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu, acc));
+  PGNN_LAUNCH_CHECK();
+  PGNN_CUDA(pgnn_launch(k_bn_bwd_finalize, dim3((unsigned)ceil_div(C, 128)), dim3(128), 0, st, acc, (int)M, (int)C, ggamma, gbeta, c1, c2));
+  PGNN_LAUNCH_CHECK();
+  if (dr)
+    PGNN_CUDA(pgnn_launch(k_bn_bwd_apply_drop, dim3(grid_items(M * C, 256)), dim3(256), 0, st, gy, ldgy, x, ldx, M, (int)C, gamma, beta, save_mean,
+                          save_invstd, relu, c1, c2, gx, ldgx, *dr));
+  else
+    PGNN_CUDA(pgnn_launch(k_bn_bwd_apply, dim3(grid_items(M * C, 256)), dim3(256), 0, st, gy, ldgy, x, ldx, M, (int)C, gamma, beta, save_mean, save_invstd, relu,
+                                                          c1, c2, gx, ldgx));
+  PGNN_LAUNCH_CHECK();
+  return PGNN_OK;
+}
+
+extern "C" {
+
+int64_t pgnn_bn_workspace_bytes(int64_t M, int64_t C) {
+  if (M < 0 || C <= 0) return PGNN_EINVAL;
+  return align_up(2 * C * 8, 256) + align_up(2 * C * 4, 256);
+}
+
+int pgnn_bn_fwd_train(const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma, const float* beta,
+                      float* running_mean, float* running_var, int64_t* num_batches_tracked, float momentum, float eps, int relu,
+                      float* y, int64_t ldy, float* save_mean, float* save_invstd, float* scale, float* shift, void* workspace,
+                      int64_t workspace_bytes, void* stream) {
+  return pgnn_internal_bn_fwd_train(x, ldx, M, C, gamma, beta, running_mean, running_var, num_batches_tracked, momentum, eps, relu, y, ldy,
+                                    save_mean, save_invstd, scale, shift, workspace, workspace_bytes, stream, nullptr);
 }
 
 int pgnn_bn_fwd_eval(const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma, const float* beta,
@@ -572,35 +794,8 @@ int pgnn_bn_fwd_eval(const float* x, int64_t ldx, int64_t M, int64_t C, const fl
 int pgnn_bn_bwd(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma,
                 const float* beta, const float* save_mean, const float* save_invstd, int relu, float* gx, int64_t ldgx,
                 float* ggamma, float* gbeta, void* workspace, int64_t workspace_bytes, void* stream) {
-  PGNN_CHECK_ARG(M > 0 && C > 0 && M < (1ll << 31) && gy && x && gamma && beta && save_mean && save_invstd && gx && workspace);
-  if (workspace_bytes < pgnn_bn_workspace_bytes(M, C)) return PGNN_EWORKSPACE;
-  cudaStream_t st = as_stream(stream);
-  double* acc = reinterpret_cast<double*>(workspace);
-  float* c1 = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + align_up(2 * C * 8, 256));
-  float* c2 = c1 + C;
-  PGNN_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * 2 * C, st));
-  {
-    auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-    if (bn_v4_enabled() && C % 4 == 0 && ldgy % 4 == 0 && ldx % 4 == 0 && ldgx % 4 == 0 && a16(gy) && a16(x) && a16(gx) && a16(gamma) && a16(beta) &&
-        a16(save_mean) && a16(save_invstd)) {
-      dim3 gv((unsigned)ceil_div(C, 128), (unsigned)ceil_div(M, kVecRows));
-      PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_v4, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu, acc));
-      PGNN_LAUNCH_CHECK();
-      PGNN_CUDA(pgnn_launch(k_bn_bwd_apply_colsum_v4, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd,
-                            relu, (const double*)acc, ggamma, gbeta, gx, ldgx, (float*)nullptr));
-      PGNN_LAUNCH_CHECK();
-      return PGNN_OK;
-    }
-  }
-  dim3 g1((unsigned)ceil_div(C, 32), (unsigned)ceil_div(M, kStatRows));
-  PGNN_CUDA(pgnn_launch(k_bn_bwd_stats, dim3(g1), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu, acc));
-  PGNN_LAUNCH_CHECK();
-  PGNN_CUDA(pgnn_launch(k_bn_bwd_finalize, dim3((unsigned)ceil_div(C, 128)), dim3(128), 0, st, acc, (int)M, (int)C, ggamma, gbeta, c1, c2));
-  PGNN_LAUNCH_CHECK();
-  PGNN_CUDA(pgnn_launch(k_bn_bwd_apply, dim3(grid_items(M * C, 256)), dim3(256), 0, st, gy, ldgy, x, ldx, M, (int)C, gamma, beta, save_mean, save_invstd, relu,
-                                                        c1, c2, gx, ldgx));
-  PGNN_LAUNCH_CHECK();
-  return PGNN_OK;
+  return pgnn_internal_bn_bwd(gy, ldgy, x, ldx, M, C, gamma, beta, save_mean, save_invstd, relu, gx, ldgx, ggamma, gbeta, workspace,
+                              workspace_bytes, stream, nullptr);
 }
 
 int pgnn_relu_fwd(const float* x, int64_t ldx, int64_t M, int64_t C, float* y, int64_t ldy, void* stream) {

@@ -20,13 +20,6 @@
 
 namespace {
 
-__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t seed, uint64_t idx) {
-  uint64_t z = seed + (idx + 1ull) * 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
 __device__ __forceinline__ int64_t mask_count(int64_t n, double rate) { return n > 0 ? (int64_t)((double)n * rate + 1.0) : 0; }
 
 // mask_off[0..B] = exclusive scan of the per-graph sample sizes (one CTA, any B; B is a few hundred)

@@ -377,6 +377,41 @@ def relu(x):
     return _Relu.apply(x)
 
 
+class _Dropout(Function):
+    @staticmethod
+    def forward(ctx, x, p, seed, layer):
+        _dev(x)
+        x = _f32(x)
+        if x.dim() != 2:
+            raise PgnnError("dropout takes [N, C] activations")
+        M, C = x.shape
+        y = torch.empty(M, C, dtype=torch.float32, device=x.device)
+        check(lib.pgnn_dropout_fwd(_p(x), x.stride(0), M, C, float(p), int(seed), int(layer), _p(y), C, _st()), "dropout_fwd")
+        ctx.args = (float(p), int(seed), int(layer))
+        return y
+
+    @staticmethod
+    def backward(ctx, g):
+        g = _f32(g)
+        M, C = g.shape
+        gx = torch.empty(M, C, dtype=torch.float32, device=g.device)
+        check(lib.pgnn_dropout_bwd(_p(g), g.stride(0), M, C, *ctx.args, _p(gx), C, _st()), "dropout_bwd")
+        return gx, None, None, None
+
+
+def dropout(x, p, seed, layer):
+    """F.dropout(x, p, training=True) (chem/model.py:271-275, bio/model.py:283-286) with the library's defined draw: element (i, c)
+    of `layer`'s [N, C] activation is kept iff splitmix64(seed, (layer << 40) | (i * C + c)) >> 32 >= floor(p * 2^32), and scaled by
+    1 / (1 - p) (include/pgnn_b200.h, pgnn_dropout_fwd).  The backward regenerates the mask from (seed, layer)."""
+    return _Dropout.apply(x, p, seed, layer)
+
+
+def draw_seed():
+    """One 62-bit dropout seed from torch's default CPU generator: a host operation (no device synchronisation), so
+    torch.manual_seed(...) makes a training run's masks reproducible."""
+    return int(torch.randint(0, 1 << 62, (), dtype=torch.int64))
+
+
 class _L2Norm(Function):
     @staticmethod
     def forward(ctx, x):
@@ -644,7 +679,7 @@ def gat(xl, att, T, edge_attr, graph, bias, heads=2, slope=0.2, is_bio=False):
 
 
 # ------------------------------------------------------------------------------------------------
-# whole-encoder fast path: chem GIN (pgnn_chem_gin_*) and GCN / GraphSAGE / GAT (pgnn_chem_conv_*)
+# whole-encoder fast path: chem GIN / GCN / GraphSAGE / GAT with dropout (pgnn_chem_encoder_*)
 # ------------------------------------------------------------------------------------------------
 import ctypes as _ct
 
@@ -664,8 +699,8 @@ def _layer_params(gnn_type, conv):
 
 class ChemEncoderPlan:
     """Per-module bookkeeping for the whole-encoder chem GNN: parameter order, gradient layout, pointer tables, and the C calls.
-    GIN runs on pgnn_chem_gin_*, gcn | graphsage | gat on pgnn_chem_conv_*; the plan's methods are the only code that tells them
-    apart."""
+    Every type runs on pgnn_chem_encoder_* (type code 0 = GIN, else PGNN_CONV_*); GIN's layout queries are pgnn_chem_gin_*, the
+    conv types' pgnn_chem_conv_*.  The plan's methods are the only code that tells them apart."""
 
     def __init__(self, gnn, gnn_type):
         self.gnn_type = gnn_type
@@ -725,21 +760,14 @@ class ChemEncoderPlan:
             self._ws_alloc = ((need + need // 16) + (16 << 20) - 1) // (16 << 20) * (16 << 20)
         return self._ws_alloc
 
-    def forward(self, ptrs, rm, rv, nbt, x, ei, ea, N, E, training, momentum, eps, out, ws, wsb):
-        args = (ptrs, rm, rv, nbt, _p(x), _p(ei), _p(ea), N, E, self.L, self.D, int(training), float(momentum), float(eps),
-                _precision, _p(out), self.D, _p(ws), wsb, _st())
-        if self.conv:
-            check(lib.pgnn_chem_conv_forward(self.conv, *args), "chem_conv_forward")
-        else:
-            check(lib.pgnn_chem_gin_forward(*args), "chem_gin_forward")
+    def forward(self, ptrs, rm, rv, nbt, x, ei, ea, N, E, training, momentum, eps, drop_p, drop_seed, out, ws, wsb):
+        check(lib.pgnn_chem_encoder_forward(self.conv, ptrs, rm, rv, nbt, _p(x), _p(ei), _p(ea), N, E, self.L, self.D, int(training),
+                                            float(momentum), float(eps), float(drop_p), int(drop_seed), _precision, _p(out), self.D,
+                                            _p(ws), wsb, _st()), "chem_encoder_forward")
 
-    def backward(self, ptrs, g, x, ea, N, E, flat, ws, wsb):
-        if self.conv:
-            check(lib.pgnn_chem_conv_backward(self.conv, ptrs, _p(g), g.stride(0), _p(x), _p(ea), N, E, self.L, self.D, _precision,
-                                              _p(flat), _p(ws), wsb, _st()), "chem_conv_backward")
-        else:
-            check(lib.pgnn_chem_gin_backward(ptrs, _p(g), g.stride(0), _p(x), N, E, self.L, self.D, _precision, _p(flat), _p(ws),
-                                             wsb, _st()), "chem_gin_backward")
+    def backward(self, ptrs, g, x, ea, N, E, drop_p, drop_seed, flat, ws, wsb):
+        check(lib.pgnn_chem_encoder_backward(self.conv, ptrs, _p(g), g.stride(0), _p(x), _p(ea), N, E, self.L, self.D, float(drop_p),
+                                             int(drop_seed), _precision, _p(flat), _p(ws), wsb, _st()), "chem_encoder_backward")
 
 
 def _deliver_flat_grads(plan, ctx, run):
@@ -755,7 +783,7 @@ def _deliver_flat_grads(plan, ctx, run):
     params = plan.params
     sole = plan.live_forwards == 1
     plan.live_forwards = max(plan.live_forwards - 1, 0)
-    needs = ctx.needs_input_grad[5:]
+    needs = ctx.needs_input_grad[_ENC_ARGS:]
     clean = sole and all(p.grad is None for p in params)
     if clean and plan.direct_grads and all(needs) and all(p.is_leaf for p in params):
         flat = plan.grad_buffer
@@ -770,7 +798,7 @@ def _deliver_flat_grads(plan, ctx, run):
         plan.last_flat_grad = flat
         for p, v in zip(params, cache[1]):
             p.grad = v
-        return (None,) * (5 + len(params))
+        return (None,) * (_ENC_ARGS + len(params))
     if plan.grad_buffer is not None and clean:
         flat = plan.grad_buffer
     else:
@@ -778,7 +806,7 @@ def _deliver_flat_grads(plan, ctx, run):
     run(flat)
     plan.last_flat_grad = flat
     grads = [v.view(s) for v, s in zip(flat.split(plan.sizes), plan.shapes)]
-    return (None, None, None, None, None) + tuple(gr if need else None for gr, need in zip(grads, needs))
+    return (None,) * _ENC_ARGS + tuple(gr if need else None for gr, need in zip(grads, needs))
 
 
 def _release_ctx(ctx):
@@ -791,9 +819,12 @@ def _release_ctx(ctx):
     ctx.released = True
 
 
+_ENC_ARGS = 7  # _ChemEncoder.forward's arguments in front of the parameters
+
+
 class _ChemEncoder(Function):
     @staticmethod
-    def forward(ctx, plan, x, edge_index, edge_attr, training, *params):
+    def forward(ctx, plan, x, edge_index, edge_attr, training, drop_p, drop_seed, *params):
         _dev(x, edge_index, edge_attr, *params)
         if x.dtype != torch.int64 or x.dim() != 2 or x.shape[1] != 2:
             raise PgnnError("chem node features must be int64 [N, 2]")
@@ -818,12 +849,13 @@ class _ChemEncoder(Function):
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
         out = torch.empty(N, D, dtype=torch.float32, device=dev)
         mom = bns[0].momentum if bns[0].momentum is not None else 0.1
-        plan.forward(ptrs, rm, rv, nbt, x, ei, ea, N, E, training, mom, bns[0].eps, out, ws, wsb)
+        plan.forward(ptrs, rm, rv, nbt, x, ei, ea, N, E, training, mom, bns[0].eps, drop_p, drop_seed, out, ws, wsb)
         ctx.plan, ctx.ws, ctx.wsb, ctx.ptrs, ctx.x, ctx.ea, ctx.dims, ctx.training = plan, ws, wsb, ptrs, x, ea, (N, E), training
+        ctx.drop = (drop_p, drop_seed)  # the backward regenerates the masks from these
         ctx.keep = params  # the pointer table refers to these storages
         if training and plan.keep_workspace:
             plan.last_ws = (ws, (N, E, plan.L, D))
-        if training and any(ctx.needs_input_grad[5:]):
+        if training and any(ctx.needs_input_grad[_ENC_ARGS:]):
             plan.live_forwards += 1
         if _VALIDATE:
             raise_on_device_errors()
@@ -839,13 +871,15 @@ class _ChemEncoder(Function):
         plan = ctx.plan
         N, E = ctx.dims
         g = _f32(g)
-        out = _deliver_flat_grads(plan, ctx, lambda flat: plan.backward(ctx.ptrs, g, ctx.x, ctx.ea, N, E, flat, ctx.ws, ctx.wsb))
+        out = _deliver_flat_grads(plan, ctx, lambda flat: plan.backward(ctx.ptrs, g, ctx.x, ctx.ea, N, E, *ctx.drop, flat, ctx.ws, ctx.wsb))
         _release_ctx(ctx)
         return out
 
 
-def chem_encoder(plan: ChemEncoderPlan, x, edge_index, edge_attr, training: bool):
-    return _ChemEncoder.apply(plan, x, edge_index, edge_attr, training, *plan.params)
+def chem_encoder(plan: ChemEncoderPlan, x, edge_index, edge_attr, training: bool, drop_p: float = 0.0, drop_seed: int = 0):
+    """The whole chem encoder in one call per pass.  With training and drop_p > 0, layer l's output carries the ops.dropout mask
+    of (drop_p, drop_seed, l): the same mask the layer-by-layer composition applies under the same seed."""
+    return _ChemEncoder.apply(plan, x, edge_index, edge_attr, training, float(drop_p), int(drop_seed), *plan.params)
 
 
 def chem_gin_relu_masks(plan: ChemEncoderPlan, gnn):

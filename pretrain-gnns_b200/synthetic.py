@@ -107,6 +107,17 @@ def mask_atoms(batch: dict, seed: int, rate: float = 0.15, mask_edge: bool = Fal
     return out
 
 
+def finetune_batch(num_graphs: int, seed: int, num_tasks: int = 12, missing_rate: float = 0.2) -> dict:
+    """chem/finetune.py's input: a zinc_batch plus `y [B, T] int64` in {-1, 0, +1} (chem/loader.py's MoleculeNet labels: +-1 a
+    label, 0 a missing one, about `missing_rate` of them)."""
+    out = zinc_batch(num_graphs, seed)
+    rng = np.random.default_rng(seed + 2750159)
+    y = np.where(rng.random((num_graphs, num_tasks)) < 0.5, 1, -1)
+    y[rng.random((num_graphs, num_tasks)) < missing_rate] = 0
+    out["y"] = _t(y)
+    return out
+
+
 def substruct_context_batch(num_graphs: int, seed: int) -> dict:
     """Config 3 (chem/pretrain_contextpred.py): substructure graphs + context graphs + overlap ids."""
     sub = zinc_batch(num_graphs, seed * 2 + 1, n_lo=12, n_hi=22)

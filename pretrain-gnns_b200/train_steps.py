@@ -9,6 +9,8 @@ restatement of the same bodies (oracle/steps_oracle.py) and with the reference's
     MaskingStep        chem/pretrain_masking.py:46-70     GNN(5,300,gnn_type) + Linear(300,119), CE on fp64 logits
     ContextPredStep    chem/pretrain_contextpred.py:50-97 GNN(5,300) + GNN(3,300), cbow / mean pooling, BCE on fp64 scores
     BioSupervisedStep  bio/pretrain_supervised.py:25-42   bio GNN_graphpred(5,300,T=5000), BCE on fp64 logits
+    FinetuneStep       chem/finetune.py:27-46             chem GNN_graphpred(5,300,T=12) with dropout 0.5, masked BCE on fp64
+                                                          logits (not a bench.py config: it is not in CONFIGS)
 """
 from __future__ import annotations
 
@@ -33,6 +35,8 @@ MASKING_KEYS = ("x", "edge_index", "edge_attr", "masked_atom_indices")
 CONTEXT_KEYS = ("x_substruct", "edge_index_substruct", "edge_attr_substruct", "center_substruct_idx", "x_context", "edge_index_context",
                 "edge_attr_context", "overlap_context_substruct_idx", "batch_overlapped_context")
 BIO_KEYS = ("x", "edge_index", "edge_attr", "batch", "center_node_idx", "go_target_pretrain")
+FINETUNE_KEYS = ("x", "edge_index", "edge_attr", "batch", "y")
+FINETUNE_SEED = 5  # seed = 5 * 1000 + 1000 * rank + batch index, in the scheme of make_batches
 
 
 def make_batches(config, rank, count, batch_size=None, num_tasks=5000):
@@ -193,6 +197,39 @@ class BioSupervisedStep(_Step):
         self.zero_grad()
         pred = self.model(types.SimpleNamespace(**b))
         loss = ops.bce_with_logits(pred, b["go_target_pretrain"].view(pred.shape))
+        loss.backward()
+        return loss
+
+
+class FinetuneStep(_Step):
+    """chem/finetune.py:27-46 with the script's defaults (num_layer 5, emb_dim 300, JK last, dropout_ratio 0.5, graph_pooling
+    mean, batch_size 32; T = 12 tasks is tox21): pred = model(x, edge_index, edge_attr, batch); loss = BCEWithLogits(pred.double(),
+    (y+1)/2) over the entries with y != 0, divided by their number.  The dropout masks come from the library's draw, one seed per
+    forward from torch's default generator (torch.manual_seed makes a run reproducible)."""
+    def __init__(self, device, gnn_type="gin", batch_size=32, num_tasks=12, drop_ratio=0.5):
+        self.graphs_per_batch, self.num_tasks = batch_size, num_tasks
+        self.model = chem.GNN_graphpred(NUM_LAYER, EMB, num_tasks, JK="last", drop_ratio=drop_ratio, graph_pooling="mean",
+                                        gnn_type=gnn_type).to(device).train()
+        self.modules = [self.model]
+        self.workload = ("chem finetune 5-layer %s emb_dim=300 dropout=%g batch_size=%d T=%d"
+                         % (gnn_type.upper() if gnn_type != "graphsage" else "GraphSAGE", drop_ratio, batch_size, num_tasks))
+
+    KEYS = FINETUNE_KEYS
+
+    def make_batches(self, rank, count):
+        return [_fields(syn.finetune_batch(self.graphs_per_batch, FINETUNE_SEED * 1000 + 1000 * rank + i, self.num_tasks), FINETUNE_KEYS)
+                for i in range(count)]
+
+    def flat_sources(self):
+        return [self.model.gnn]
+
+    def named_modules(self):
+        return {"model": self.model}
+
+    def __call__(self, b):
+        self.zero_grad()
+        pred = self.model(b["x"], b["edge_index"], b["edge_attr"], b["batch"])
+        loss = ops.masked_bce_with_logits(pred, b["y"].view(pred.shape))
         loss.backward()
         return loss
 
