@@ -11,13 +11,20 @@
 //   wgrad  gw[N,K] = gy[M,N]^T . x[M,K]      A MN-major, B MN-major (node rows are the reduction; split-K)
 //
 // Structure (per CTA: one 128 x BN output tile, two warpgroups of 64 rows each, BK = 32 per block):
-//   * every thread loads its share of the next block (16-byte global loads along whichever extent is contiguous,
-//     zero-filled out of range) into registers while the tensor cores work on the current one;
-//   * it then splits the values into hi / lo and stores both into the other shared-memory stage in the
-//     K-major 128B-swizzled layout (tf32 wgmma reads K-major operands only, so MN-major sources are transposed
-//     on this store), and fences the stores to the async proxy;
-//   * per block and warpgroup: 4 k-steps x (BN / 64) column halves x 3 products of wgmma.m64n64k8; the hi*hi chain
-//     and the cross terms go to separate register accumulators;
+//   * A comes from registers (the RS form of wgmma): each thread holds its rows of the tf32 A fragment and splits them
+//     into hi / lo in registers.  Block kb + 1 of A is copied raw into the other of two shared-memory buffers with
+//     cp.async while block kb runs (no registers held by the copy), and read from there into the fragment.  Within a block
+//     the reduction index is permuted (kperm) so that a thread's fragment slots are two 16-byte pieces of each of its
+//     rows: one 16-byte shared-memory read per row and two k-steps for a K-major A; an MN-major A (wgrad's gy^T) is read
+//     element by element.
+//   * B goes through NSTAGE shared-memory stages: every thread loads its share of block kb + 1 (16-byte global loads
+//     along whichever extent is contiguous, zero-filled out of range) while the tensor cores work on block kb, then
+//     splits it into hi / lo and stores both, permuted like A, in the K-major 128B-swizzled layout (tf32 wgmma reads a
+//     K-major B only, so an MN-major source is transposed on this store), and fences the stores to the async proxy;
+//   * per k-step and warpgroup: one commit group of 3 wgmma.m64nBNk8 (lo*hi, hi*lo into the cross-term accumulator,
+//     hi*hi into its own), A fragments in FRAG_SETS register sets.  A set is rewritten only after wait_group has
+//     retired the group that read it, so FRAG_SETS - 1 groups stay queued across k-steps, k-blocks and the one barrier
+//     per block; with three B stages that barrier is also what frees the stage the next block is stored into;
 //   * epilogue: both accumulators are summed into a shared-memory staging tile, then written out row-contiguously
 //     with bias / ReLU / mask applied, plus the optional fused column reductions.
 #include <cstdlib>
@@ -44,30 +51,81 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// at most N of this warpgroup's commit groups still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// d[64 x 64] += a[64 x 8] . b[64 x 8]^T, tf32 operands from shared memory, fp32 accumulators in registers
-__device__ __forceinline__ void wgmma_tf32_m64n64k8(float (&d)[32], uint64_t da, uint64_t db) {
+// d[64 x 64] += a[64 x 8] . b[64 x 8]^T: tf32 A fragment from registers, B from shared memory, fp32 accumulators in registers
+__device__ __forceinline__ void wgmma_tf32_m64n64k8_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
       "setp.ne.b32 p, 1, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t"
       "}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
         "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
         "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
         "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db)
       : "memory");
 }
-// keeps the compiler from moving accumulator registers across the asynchronous wgmma window
-__device__ __forceinline__ void fence_acc(float (&d)[32]) {
-#pragma unroll
-  for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
+// d[64 x 128] += a[64 x 8] . b[128 x 8]^T, as above
+__device__ __forceinline__ void wgmma_tf32_m64n128k8_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db)
+      : "memory");
 }
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[BN / 2], const uint32_t (&a)[4], uint64_t db) {
+  if constexpr (BN == 128) wgmma_tf32_m64n128k8_rs(d, a, db);
+  else wgmma_tf32_m64n64k8_rs(d, a, db);
+}
+// keeps the compiler from moving accumulator registers across the asynchronous wgmma window
+template <int R>
+__device__ __forceinline__ void fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// The reduction index k of a block and its slot in the A fragment and the stored B tile: the two base-4 digits of k mod 16
+// swap (an involution, so it also maps a slot back to its k).  k-step j, fragment column c (thread t = c mod 4 of its quad)
+// then holds k = 16 (j / 2) + 4 t + 2 (j % 2) + c / 4: thread t's slots are k = 4t .. 4t + 3 and 16 + 4t .. 16 + 4t + 3.
+__device__ __forceinline__ int kperm(int k) { return (k & 16) | ((k & 3) << 2) | ((k >> 2) & 3); }
+
+// float offset of element (m, k) of a raw MN-major A block [BK][BM].  The XOR keeps 4-row pieces contiguous and spreads both
+// the loader's 16-byte stores (k and k + 1) and the fragment reads (8 rows x 4 threads of a quad) over all 32 banks.
+__device__ __forceinline__ int araw_off(int m, int k) { return k * BM + (m ^ ((((k >> 2) & 3) << 3) ^ ((k & 1) << 4))); }
+
+// float offset of element (m, k) of a raw K-major A block [BM][BK]: 16-byte pieces stay whole, and the piece index is XOR-ed with
+// 4 (m & 1), so the fragment's 16-byte reads (rows m, m + 1 x the 4 threads of a quad per quarter warp) hit 8 distinct pieces
+__device__ __forceinline__ int akc_off(int m, int k) { return m * BK + ((((k >> 2) ^ ((m & 1) << 2))) << 2) + (k & 3); }
+
+// 16-byte global -> shared copy that bypasses the registers; the destination bytes from `bytes` on are zero-filled (0: nothing
+// is read)
+__device__ __forceinline__ void cp_async16(float* dst, const float* src, int bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
 __device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
@@ -84,10 +142,25 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
 // as a NaN, so a +-Inf there is the fp32 result.
 __device__ __forceinline__ float sum_chains(float acc, float accx) { return isinf(acc) ? acc : acc + accx; }
 
+// p[0 .. 3] with the elements from index n on zero (n <= 0: all zero); one 16-byte load when all four are in range
+__device__ __forceinline__ float4 ldg4_tail(const float* p, int n) {
+  float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (n > 3) x = __ldg(reinterpret_cast<const float4*>(p));
+  else if (n > 0) {
+    x.x = __ldg(p);
+    if (n > 1) x.y = __ldg(p + 1);
+    if (n > 2) x.z = __ldg(p + 2);
+  }
+  return x;
+}
+
+__device__ __forceinline__ float f4_at(const float4& v, int i) { return i == 0 ? v.x : i == 1 ? v.y : i == 2 ? v.z : v.w; }
+
 // Operand tile loader.  KC: source contiguous along the reduction (element (r,k) at src[r*ld + k]); otherwise contiguous
 // along the row index (element (r,k) at src[k*ld + r]).  R = rows (MN extent) of the tile.  Each thread owns NV 16-byte
 // pieces of a [R x BK] block.  MN-major pieces are assigned so that a warp covers 16 rows x 8 k: 64-byte global segments,
-// and the transposing scalar stores spread over 16 banks.
+// and the transposing scalar stores spread over 16 banks.  The permuted K-major stores (one scalar per element) hit
+// 32 distinct banks per warp.
 template <bool KC, int R>
 struct Loader {
   static constexpr int NV = R * BK / 4 / NTHREADS;
@@ -124,66 +197,66 @@ struct Loader {
       const int gr = r0 + rr;
       float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
       if (KC) {
-        if (gr < rows) {
-          const float* p = blk + (int64_t)gr * ld + kk;
-          if (kk + 3 < krem) x = __ldg(reinterpret_cast<const float4*>(p));
-          else if (kk < krem) {
-            x.x = __ldg(p);
-            if (kk + 1 < krem) x.y = __ldg(p + 1);
-            if (kk + 2 < krem) x.z = __ldg(p + 2);
-          }
-        }
+        if (gr < rows) x = ldg4_tail(blk + (int64_t)gr * ld + kk, krem - kk);
       } else if (kk < krem && gr < rows) {
-        const float* p = blk + (int64_t)kk * ld + gr;
-        if (gr + 3 < rows) x = __ldg(reinterpret_cast<const float4*>(p));
-        else {
-          x.x = __ldg(p);
-          if (gr + 1 < rows) x.y = __ldg(p + 1);
-          if (gr + 2 < rows) x.z = __ldg(p + 2);
-        }
+        x = ldg4_tail(blk + (int64_t)kk * ld + gr, rows - gr);
       }
       v[i] = x;
     }
   }
+  // B: hi / lo into the K-major swizzled tile, element k at slot kperm(k)
   __device__ __forceinline__ void store(uint8_t* hi, uint8_t* lo) const {
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
       int rr, kk;
       piece(threadIdx.x + i * NTHREADS, rr, kk);
-      if (KC) {
-        float4 h, l;
-        split_tf32(v[i].x, h.x, l.x);
-        split_tf32(v[i].y, h.y, l.y);
-        split_tf32(v[i].z, h.z, l.z);
-        split_tf32(v[i].w, h.w, l.w);
-        const int o = sw128_off(rr, kk);
-        *reinterpret_cast<float4*>(hi + o) = h;
-        *reinterpret_cast<float4*>(lo + o) = l;
-      } else {
-        const float xv[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
+      if (!KC) asm volatile("" : "+r"(rr), "+r"(kk));  // recompute the 4 NV store offsets per block rather than hold them in registers
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float h, l;
-          split_tf32(xv[q], h, l);
-          const int o = sw128_off(rr + q, kk);
-          *reinterpret_cast<float*>(hi + o) = h;
-          *reinterpret_cast<float*>(lo + o) = l;
-        }
+      for (int q = 0; q < 4; ++q) {
+        float h, l;
+        split_tf32(f4_at(v[i], q), h, l);
+        const int o = KC ? sw128_off(rr, kperm(kk + q)) : sw128_off(rr + q, kperm(kk));
+        *reinterpret_cast<float*>(hi + o) = h;
+        *reinterpret_cast<float*>(lo + o) = l;
       }
     }
   }
 };
 
+// A: block kb of this CTA's 128 rows copied raw into a shared-memory buffer (akc_off / araw_off layout) with cp.async, so the
+// copy in flight holds no registers.  Same pieces as Loader<KC, BM>; out-of-range elements are zero-filled.
+template <bool KC>
+__device__ __forceinline__ void a_copy(float* dst, const float* __restrict__ A, int64_t lda, int m0, int M, int k0, int krem) {
+#pragma unroll
+  for (int i = 0; i < Loader<KC, BM>::NV; ++i) {
+    int rr, kk;
+    Loader<KC, BM>::piece(threadIdx.x + i * NTHREADS, rr, kk);
+    const int gr = m0 + rr;
+    int n = 0;  // elements of the piece in range
+    if (KC) n = gr < M ? min(max(krem - kk, 0), 4) : 0;
+    else n = kk < krem ? min(max(M - gr, 0), 4) : 0;
+    const float* src = n > 0 ? (KC ? A + (int64_t)gr * lda + k0 + kk : A + (int64_t)(k0 + kk) * lda + gr) : A;
+    cp_async16(dst + (KC ? akc_off(rr, kk) : araw_off(rr, kk)), src, 4 * n);
+  }
+  cp_async_commit();
+}
+
+constexpr int NSTAGE = 3;  // B stages: block kb + 1 is stored while blocks kb - 1 and kb may still be read
+
 template <int BN>
 struct TileCfg {
-  static constexpr int A_BYTES = BM * BK * 4;  // 16 KiB per buffer
   static constexpr int B_BYTES = BN * BK * 4;
-  static constexpr int STAGE = 2 * (A_BYTES + B_BYTES);  // [A hi | A lo | B hi | B lo]
-  static constexpr int SLD = BN + 4;                     // epilogue staging row stride (16-byte aligned rows)
+  static constexpr int STAGE = 2 * B_BYTES;      // [B hi | B lo]
+  static constexpr int A_RAW = BM * BK * 4;      // one raw A block (16 KiB), two buffers
+  static constexpr int SLD = BN + 4;             // epilogue staging row stride (16-byte aligned rows)
   static constexpr int EPI = BM * SLD * 4 + BM * kMaxHookQ * 4;  // staging tile + the hooks' [128][Q <= 16] slice
-  static constexpr int RING = 2 * STAGE;
+  static constexpr int RING = NSTAGE * STAGE + 2 * A_RAW;
   static constexpr int SMEM = (RING > EPI ? RING : EPI) + 1024;  // + alignment slack of the 1024-byte swizzle atoms
-  // two CTAs per SM at BN = 64 (96 KiB of stages, <= 128 registers), one at BN = 128
+  // A-fragment register sets (8 registers each) in rotation: FRAG_SETS - 1 of the warpgroup's commit groups stay queued
+  // while the next is prepared
+  static constexpr int FRAG_SETS = BN == 128 ? 4 : 2;
+  // Two CTAs per SM at BN = 64: 128 registers (sm_90a, 0 spills) and 81 KiB of shared memory each.  One at BN = 128:
+  // 223-242 registers, 129 KiB.
   static constexpr int MIN_BLOCKS = BN <= 64 ? 2 : 1;
 };
 
@@ -300,19 +373,21 @@ template <bool A_KC, bool B_KC, int BN>
 __global__ void __launch_bounds__(NTHREADS, TileCfg<BN>::MIN_BLOCKS)
 k_gemm_3xtf32(const float* __restrict__ A, int64_t lda, const float* __restrict__ B, int64_t ldb, float* __restrict__ C, int64_t ldc,
               int M, int N, int K, int k_per_split, TcEpilogue ep) {
-  static_assert(BN % 64 == 0 && BN <= 128, "column halves of 64 (wgmma N); two accumulators of BN / 2 registers each");
+  static_assert(BN == 64 || BN == 128, "one wgmma.m64nBNk8 per product; two accumulators of BN / 2 registers each");
   using Cfg = TileCfg<BN>;
-  constexpr int NH = BN / 64;
+  constexpr int NF = Cfg::FRAG_SETS;
+  static_assert((BK / 8) % NF == 0, "k-step j uses fragment set j % NF in every block");
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(16) float s_bias[BN];
   // the swizzle pattern is a function of the address bits: stages start on 1024-byte boundaries
   uint8_t* smem = smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023);
-  auto a_hi = [&](int s) { return smem + s * Cfg::STAGE; };
-  auto a_lo = [&](int s) { return a_hi(s) + Cfg::A_BYTES; };
-  auto b_hi = [&](int s) { return a_hi(s) + 2 * Cfg::A_BYTES; };
+  auto b_hi = [&](int s) { return smem + s * Cfg::STAGE; };
   auto b_lo = [&](int s) { return b_hi(s) + Cfg::B_BYTES; };
+  float* a_raw = reinterpret_cast<float*>(smem + NSTAGE * Cfg::STAGE);  // two raw A blocks
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
+  const int t = lane & 3;
+  const int mrow = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's A-fragment rows: mrow and mrow + 8
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
   const int kbeg = blockIdx.z * k_per_split;
   const int kend = min(K, kbeg + k_per_split);
@@ -322,76 +397,86 @@ k_gemm_3xtf32(const float* __restrict__ A, int64_t lda, const float* __restrict_
   pdl_prologue();
   for (int i = threadIdx.x; i < BN; i += NTHREADS) s_bias[i] = (s_bias_on && n0 + i < N) ? ep.bias[n0 + i] : 0.f;
 
-  Loader<A_KC, BM> la;
   Loader<B_KC, BN> lb;
-  la.init(A, lda, m0, M, kbeg);
   lb.init(B, ldb, n0, N, kbeg);
 
-  float acc[NH][32], accx[NH][32];  // hi*hi chain | cross terms
+  float acc[BN / 2], accx[BN / 2];  // hi*hi chain | cross terms
 #pragma unroll
-  for (int h = 0; h < NH; ++h)
-#pragma unroll
-    for (int i = 0; i < 32; ++i) acc[h][i] = accx[h][i] = 0.f;
+  for (int i = 0; i < BN / 2; ++i) acc[i] = accx[i] = 0.f;
+  uint32_t fh[NF][4], fl[NF][4];  // A fragment hi / lo, NF sets
 
   if (nkb > 0) {
-    la.load(0, kend - kbeg);
+    a_copy<A_KC>(a_raw, A, lda, m0, M, kbeg, kend - kbeg);
     lb.load(0, kend - kbeg);
-    la.store(a_hi(0), a_lo(0));
     lb.store(b_hi(0), b_lo(0));
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor cores
+    cp_async_wait_all();
   }
+  int s = 0;  // B stage of block kb
 #pragma unroll 1
   for (int kb = 0; kb < nkb; ++kb) {
-    const int s = kb & 1;
-    __syncthreads();  // stage s is complete; every wgmma of block kb - 1 (stage s ^ 1) has retired
+    // B stage s and A buffer kb & 1 are complete.  Every thread has retired its warpgroup's groups of block kb - 2 (at most
+    // NF - 1 groups are in flight after a wait), so stage (s + 1) % NSTAGE is free for block kb + 1; A buffer (kb + 1) & 1 was
+    // read by block kb - 1's fragment loads.
+    __syncthreads();
     const bool more = kb + 1 < nkb;
-    if (more) {  // next block's global loads fly under this block's MMAs
-      la.load(kb + 1, kend - kbeg - (kb + 1) * BK);
+    if (more) {  // next block's copies and global loads fly under this block's MMAs
+      a_copy<A_KC>(a_raw + ((kb + 1) & 1) * (BM * BK), A, lda, m0, M, kbeg + (kb + 1) * BK, kend - kbeg - (kb + 1) * BK);
       lb.load(kb + 1, kend - kbeg - (kb + 1) * BK);
     }
-    const uint32_t ah = smem_u32(a_hi(s)) + wg * (64 * 128), al = smem_u32(a_lo(s)) + wg * (64 * 128);
-    const uint32_t bh = smem_u32(b_hi(s)), bl = smem_u32(b_lo(s));
-    wgmma_fence();
+    const float* ar = a_raw + (kb & 1) * (BM * BK);
+    float4 av[2];  // K-major A: elements 16 (j / 2) + 4t .. + 3 of rows mrow, mrow + 8 (the slots of k-steps j, j + 1 for even j)
+    const uint64_t dh = gmma_desc_sw128(smem_u32(b_hi(s))), dl = gmma_desc_sw128(smem_u32(b_lo(s)));
 #pragma unroll
     for (int j = 0; j < BK / 8; ++j) {  // k-step j: 8 fp32 = 32 bytes into the 128-byte swizzle row
+      const int f = j % NF;
+      wgmma_wait<NF - 1>();  // the group that last read set f (k-step j - NF) has retired
+      if (A_KC && (j & 1) == 0) {
 #pragma unroll
-      for (int h = 0; h < NH; ++h) {
-        const uint32_t bo = h * (64 * 128) + j * 32;
-        wgmma_tf32_m64n64k8(accx[h], gmma_desc_sw128(al + j * 32), gmma_desc_sw128(bh + bo));
-        wgmma_tf32_m64n64k8(accx[h], gmma_desc_sw128(ah + j * 32), gmma_desc_sw128(bl + bo));
-        wgmma_tf32_m64n64k8(acc[h], gmma_desc_sw128(ah + j * 32), gmma_desc_sw128(bh + bo));
+        for (int r = 0; r < 2; ++r) av[r] = *reinterpret_cast<const float4*>(ar + akc_off(mrow + 8 * r, 16 * (j >> 1) + 4 * t));
       }
-    }
-    wgmma_commit();
-    if (more) {
-      la.store(a_hi(s ^ 1), a_lo(s ^ 1));
-      lb.store(b_hi(s ^ 1), b_lo(s ^ 1));
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    wgmma_wait_all();
+      float x[4];  // fragment rows mrow, mrow + 8 at columns t, t + 4 of the k-step
 #pragma unroll
-    for (int h = 0; h < NH; ++h) {
-      fence_acc(acc[h]);
-      fence_acc(accx[h]);
+      for (int q = 0; q < 4; ++q) {
+        const int slot = 2 * (j & 1) + (q >> 1);  // element of the thread's 4-element piece
+        if (A_KC) x[q] = f4_at(av[q & 1], slot);
+        else x[q] = ar[araw_off(mrow + 8 * (q & 1), 16 * (j >> 1) + 4 * t + slot)];
+      }
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        float h, l;
+        split_tf32(x[q], h, l);
+        fh[f][q] = __float_as_uint(h);
+        fl[f][q] = __float_as_uint(l);
+      }
+      wgmma_fence();
+      wgmma_tf32_rs<BN>(accx, fl[f], dh + 2 * j);  // + j * 32 bytes in the descriptor's 16-byte address units
+      wgmma_tf32_rs<BN>(accx, fh[f], dl + 2 * j);
+      wgmma_tf32_rs<BN>(acc, fh[f], dh + 2 * j);
+      wgmma_commit();
+    }
+    s = s + 1 == NSTAGE ? 0 : s + 1;
+    if (more) {
+      lb.store(b_hi(s), b_lo(s));
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      cp_async_wait_all();  // this thread's A copies of block kb + 1 have landed; the barrier publishes them
     }
   }
+  wgmma_wait<0>();
+  fence_acc(acc);
+  fence_acc(accx);
   __syncthreads();  // the stages are free: the staging tile reuses them
 
   // accumulator fragment of wgmma m64nN (f32): register 4i + j of lane l in warp w of the warpgroup holds
   // row 16 w + l / 4 + 8 (j / 2), column 8 i + 2 (l % 4) + (j % 2)
   float* stage = reinterpret_cast<float*>(smem);
-  {
-    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-    for (int h = 0; h < NH; ++h)
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int col = h * 64 + i * 8 + (lane & 3) * 2;
-        *reinterpret_cast<float2*>(stage + row * Cfg::SLD + col) =
-            make_float2(sum_chains(acc[h][4 * i], accx[h][4 * i]), sum_chains(acc[h][4 * i + 1], accx[h][4 * i + 1]));
-        *reinterpret_cast<float2*>(stage + (row + 8) * Cfg::SLD + col) =
-            make_float2(sum_chains(acc[h][4 * i + 2], accx[h][4 * i + 2]), sum_chains(acc[h][4 * i + 3], accx[h][4 * i + 3]));
-      }
+  for (int i = 0; i < BN / 8; ++i) {
+    const int col = i * 8 + t * 2;
+    *reinterpret_cast<float2*>(stage + mrow * Cfg::SLD + col) =
+        make_float2(sum_chains(acc[4 * i], accx[4 * i]), sum_chains(acc[4 * i + 1], accx[4 * i + 1]));
+    *reinterpret_cast<float2*>(stage + (mrow + 8) * Cfg::SLD + col) =
+        make_float2(sum_chains(acc[4 * i + 2], accx[4 * i + 2]), sum_chains(acc[4 * i + 3], accx[4 * i + 3]));
   }
   __syncthreads();
   tile_epilogue<BN>(stage, s_bias, s_bias_on, m0, n0, M, N, C + (int64_t)blockIdx.z * ep.split_stride, ldc, ep);
