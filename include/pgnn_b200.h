@@ -253,6 +253,17 @@ PGNN_API int pgnn_row_gather_bwd(const float* g, int64_t ldg, const int64_t* idx
  * i.e. the gradient of the loss w.r.t. the logits.  labels: int64 [M] in [0, V). */
 PGNN_API int pgnn_softmax_ce_fwd(const float* logits, int64_t ld, int64_t M, int64_t V, const int64_t* labels,
                                  double* loss_mean, float* dlogits, int64_t lddl, void* stream);
+/* The same loss with each label given as a row of Q floats (label_rows [M, ld_label]): the label of row m is the FIRST index
+ * of the maximum of its Q values, `torch.argmax(batch.mask_edge_label, dim=1)` followed by CrossEntropyLoss of bio masking
+ * (bio/pretrain_masking.py:47-55: V = 7 edge types, Q = 9 attribute columns; evaluated in fp64).  A label >= V, or a row
+ * without a finite maximum (a NaN in it, or a +-Inf maximum), sets PGNN_DEVERR_LABEL and the row contributes its
+ * log-sum-exp only, as an out-of-range int64 label does above.  *loss_mean is OVERWRITTEN, dlogits as above.  Deterministic
+ * (per-CTA fp64 partials folded in order, no floating-point atomics).  workspace: pgnn_softmax_ce_rows_workspace_bytes()
+ * bytes, any content. */
+PGNN_API int64_t pgnn_softmax_ce_rows_workspace_bytes(void);
+PGNN_API int pgnn_softmax_ce_rows_fwd(const float* logits, int64_t ld, int64_t M, int64_t V, const float* label_rows, int64_t ld_label,
+                                      int64_t Q, double* loss_mean, float* dlogits, int64_t lddl, void* workspace,
+                                      int64_t workspace_bytes, void* stream);
 /* out[r] = sum_d a[r,d] * b[(r + shift) mod B, d]   (cycle_index negatives, pretrain_contextpred.py:36-39,64-67) */
 PGNN_API int pgnn_shifted_rowdot_fwd(const float* a, int64_t lda, const float* b, int64_t ldb, int64_t B, int64_t C,
                                      int64_t shift, float* out, void* stream);

@@ -185,6 +185,104 @@ k_softmax_ce(const float* __restrict__ logits, int64_t ld, int64_t M, int V, con
   }
 }
 
+// The same loss with the class of row m given as a row of Q floats: label = the first index of the row's maximum, what
+// `torch.argmax(batch.mask_edge_label, dim=1)` computes for bio masking (bio/pretrain_masking.py:47-55; torch >= 1.7 documents
+// the first maximal index).  That head has V = 7 and ~10^5 rows per step, so a row is held by a group of G lanes (the
+// power of two >= V, at most 32; 32 / G rows per warp) instead of a whole warp, and the loss is folded deterministically: one
+// fp64 partial per CTA, summed in CTA order by the last CTA to finish (the ticket scheme of losses.cu), no floating-point atomics.
+// A label >= V, or a label row without a finite maximum (a NaN in it, a +-Inf maximum), sets PGNN_DEVERR_LABEL and the row
+// contributes as a bad int64 label does in k_softmax_ce: its log-sum-exp only.
+constexpr int kCeRowsThreads = 256;
+constexpr int kCeRowsMaxBlocks = kNumSMs * 4;
+
+struct CeRowsWs {
+  double partial[kCeRowsMaxBlocks];
+  unsigned int ticket;
+  unsigned int pad;
+};
+
+template <int G>
+__global__ void __launch_bounds__(kCeRowsThreads)
+k_softmax_ce_rows(const float* __restrict__ logits, int64_t ld, int64_t M, int V, const float* __restrict__ lab, int64_t ldl, int Q,
+                  CeRowsWs* __restrict__ ws, double* __restrict__ loss_mean, float* __restrict__ dlogits, int64_t lddl,
+                  unsigned int* __restrict__ err) {
+  pdl_prologue();
+  constexpr int kRowsPerCta = kCeRowsThreads / G;
+  __shared__ double s_part[kCeRowsThreads / 32];
+  __shared__ bool s_last;
+  const int sub = threadIdx.x & (G - 1);
+  const double inv_m = 1.0 / (double)M;
+  double acc = 0.0;
+  bool bad = false;
+  // `base` is uniform across the CTA, so every lane of a warp runs every iteration and the group shuffles below may use the
+  // full mask; the lanes of a row past M (`live` false) only take part in the shuffles
+  for (int64_t base = (int64_t)blockIdx.x * kRowsPerCta; base < M; base += (int64_t)gridDim.x * kRowsPerCta) {
+    const int64_t r = base + threadIdx.x / G;
+    const bool live = r < M;
+    const float* row = logits + r * ld;
+    double mx = -1e300;
+    if (live)
+      for (int v = sub; v < V; v += G) mx = fmax(mx, (double)row[v]);
+#pragma unroll
+    for (int o = G / 2; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    double se = 0.0;
+    if (live)
+      for (int v = sub; v < V; v += G) se += exp((double)row[v] - mx);
+#pragma unroll
+    for (int o = G / 2; o > 0; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
+    const double lse = mx + log(se);
+    float best = -INFINITY;
+    int bi = Q, nan = 0;
+    if (live) {
+      const float* t = lab + r * ldl;
+      for (int q = sub; q < Q; q += G) {  // ascending per lane: a lane keeps its first maximum
+        const float x = t[q];
+        if (x != x) nan = 1;
+        else if (x > best) best = x, bi = q;
+      }
+    }
+#pragma unroll
+    for (int o = G / 2; o > 0; o >>= 1) {
+      const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      nan |= __shfl_xor_sync(0xffffffffu, nan, o);
+      if (ob > best || (ob == best && oi < bi)) best = ob, bi = oi;
+    }
+    int y = bi;
+    if (nan || !isfinite(best) || y >= V) {
+      bad |= live;
+      y = -1;
+    }
+    if (live) {
+      for (int v = sub; v < V; v += G) {
+        const double p = exp((double)row[v] - lse);
+        dlogits[r * lddl + v] = (float)((p - (v == y ? 1.0 : 0.0)) * inv_m);
+      }
+      for (int v = V + sub; v < lddl; v += G) dlogits[r * lddl + v] = 0.f;  // padding columns of the 16-byte-aligned row
+      if (sub == 0) acc += lse - (y >= 0 ? (double)row[y] : 0.0);
+    }
+  }
+  if (bad && err) atomicOr(err, (unsigned)PGNN_DEVERR_LABEL);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double b = 0.0;
+    for (int w = 0; w < kCeRowsThreads / 32; ++w) b += s_part[w];
+    ws->partial[blockIdx.x] = b;
+    __threadfence();
+    s_last = atomicAdd(&ws->ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (s_last && threadIdx.x == 0) {
+    __threadfence();
+    double s = 0.0;
+    for (unsigned b = 0; b < gridDim.x; ++b) s += reinterpret_cast<volatile double*>(ws->partial)[b];
+    *loss_mean = s * inv_m;
+  }
+}
+
 inline int grid_items(int64_t items, int threads) {
   int64_t b = ceil_div(items, threads);
   const int64_t cap = (int64_t)kNumSMs * 16;
@@ -255,6 +353,40 @@ int pgnn_softmax_ce_fwd(const float* logits, int64_t ld, int64_t M, int64_t V, c
   if (M == 0) return PGNN_OK;
   PGNN_CHECK_ARG(logits && labels && dlogits);
   PGNN_CUDA(pgnn_launch(k_softmax_ce, dim3(grid_items(M * 32, 256)), dim3(256), 0, st, logits, ld, M, (int)V, labels, loss_mean, dlogits, lddl, pgnn_error_flag_ptr()));
+  PGNN_LAUNCH_CHECK();
+  return PGNN_OK;
+}
+
+int64_t pgnn_softmax_ce_rows_workspace_bytes(void) { return (int64_t)sizeof(CeRowsWs); }
+
+int pgnn_softmax_ce_rows_fwd(const float* logits, int64_t ld, int64_t M, int64_t V, const float* label_rows, int64_t ld_label, int64_t Q,
+                             double* loss_mean, float* dlogits, int64_t lddl, void* workspace, int64_t workspace_bytes, void* stream) {
+  PGNN_CHECK_ARG(M >= 0 && V > 0 && V <= (1 << 30) && Q > 0 && Q <= (1 << 30) && loss_mean && lddl >= V && ld >= V && ld_label >= Q && workspace);
+  if (workspace_bytes < (int64_t)sizeof(CeRowsWs)) return PGNN_EWORKSPACE;
+  cudaStream_t st = as_stream(stream);
+  if (M == 0) {
+    PGNN_CUDA(cudaMemsetAsync(loss_mean, 0, sizeof(double), st));
+    return PGNN_OK;
+  }
+  PGNN_CHECK_ARG(logits && label_rows && dlogits);
+  CeRowsWs* ws = reinterpret_cast<CeRowsWs*>(workspace);
+  PGNN_CUDA(cudaMemsetAsync(&ws->ticket, 0, sizeof(unsigned int), st));
+  const int G = V <= 1 ? 1 : V <= 2 ? 2 : V <= 4 ? 4 : V <= 8 ? 8 : V <= 16 ? 16 : 32;
+  int64_t blocks = ceil_div(M, (int64_t)(kCeRowsThreads / G));
+  if (blocks > kCeRowsMaxBlocks) blocks = kCeRowsMaxBlocks;
+  const dim3 grid((unsigned)blocks), block(kCeRowsThreads);
+  unsigned int* err = pgnn_error_flag_ptr();
+#define PGNN_CE_ROWS(g) pgnn_launch(k_softmax_ce_rows<g>, grid, block, 0, st, logits, ld, M, (int)V, label_rows, ld_label, (int)Q, ws, loss_mean, \
+                                    dlogits, lddl, err)
+  switch (G) {
+    case 1: PGNN_CUDA(PGNN_CE_ROWS(1)); break;
+    case 2: PGNN_CUDA(PGNN_CE_ROWS(2)); break;
+    case 4: PGNN_CUDA(PGNN_CE_ROWS(4)); break;
+    case 8: PGNN_CUDA(PGNN_CE_ROWS(8)); break;
+    case 16: PGNN_CUDA(PGNN_CE_ROWS(16)); break;
+    default: PGNN_CUDA(PGNN_CE_ROWS(32)); break;
+  }
+#undef PGNN_CE_ROWS
   PGNN_LAUNCH_CHECK();
   return PGNN_OK;
 }

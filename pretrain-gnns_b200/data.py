@@ -284,16 +284,20 @@ class BioGraphStore:
         self.center = IndexLists([[int(c)] for c in center_idx], dev)
         self.pair_first = None
 
-    def extract_context(self, graph_ids_host, l1):
-        """bio ExtractSubstructureContextPair(l1, center=True) + BatchSubstructContext.from_data_list (bio/util.py:123-205,
+    def extract_context(self, graph_ids_host, l1, center=True, seed=0):
+        """bio ExtractSubstructureContextPair(l1, center) + BatchSubstructContext.from_data_list (bio/util.py:123-205,
         bio/batch.py:196-265) on the device: the substructure side is the ordinary collation of the whole ego graphs, the
-        context side holds the nodes further than l1 hops from the centre node, every one of them an overlap node.  Graphs
-        without a context are dropped by the reference; here that is reported (`kept`) and raised if it happens, because the
-        substructure side would have to be re-collated without them."""
+        context side holds the nodes further than l1 hops from the root node, every one of them an overlap node.  The root is
+        the centre node with center=True; with center=False (bio/pretrain_contextpred.py's default) it is a uniform draw per
+        graph, pgnn_extract_pairs' splitmix64(seed, batch slot) mod n (bio/util.py:159-164 uses random.sample; `seed`: a fresh
+        value per step).  center_substruct_idx is the ego centre either way (bio/util.py:172).  Graphs without a context are
+        dropped by the reference; here that is reported (`kept`) and raised if it happens, because the substructure side would
+        have to be re-collated without them."""
         ids = np.ascontiguousarray(graph_ids_host, dtype=np.int64)
         out = self.collate(ids)
-        roots = self.center.values[torch.from_numpy(ids).to(self.device)]      # one centre per graph: list_ptr = arange
-        ids_dev, ws, offsets, N, E = _extract(self, ids, roots, 0, 0, l1, 0, 1)
+        # one centre per graph: list_ptr = arange
+        roots = self.center.values[torch.from_numpy(ids).to(self.device)] if center else None
+        ids_dev, ws, offsets, N, E = _extract(self, ids, roots, seed if not center else 0, 0, l1, 0, 1)
         B, dev = len(ids), self.device
         i64, f32 = dict(dtype=torch.int64, device=dev), dict(dtype=torch.float32, device=dev)
         xc, ec, ac = torch.empty((N, 1), **f32), torch.empty((2 * E,), **i64), torch.empty((E, 9), **f32)
@@ -304,7 +308,7 @@ class BioGraphStore:
                                         sizes.data_ptr(), torch.cuda.current_stream(dev).cuda_stream), "pgnn_extract_fill_bio")
         _, _, nc, e_c, ko, kept = (int(v) for v in offsets[:, B].tolist())
         if kept != B:
-            raise ValueError("%d of %d ego graphs have no node further than l1 = %d hops from their centre" % (B - kept, B, l1))
+            raise ValueError("%d of %d ego graphs have no node further than l1 = %d hops from their root" % (B - kept, B, l1))
         return SimpleNamespace(x_substruct=out.x, edge_index_substruct=out.edge_index, edge_attr_substruct=out.edge_attr,
                                center_substruct_idx=out.center_node_idx, x_context=xc[:nc], edge_index_context=ec[:2 * e_c].view(2, e_c),
                                edge_attr_context=ac[:e_c], overlap_context_substruct_idx=ov[:ko], batch_overlapped_context=seg[:ko],

@@ -918,7 +918,10 @@ class _MaskedCE(Function):
         rep, w = _f32(node_rep), _f32(weight).contiguous()
         idx, labels = idx.contiguous(), labels.contiguous()
         idx2 = None if idx2 is None else idx2.contiguous()
-        if idx.dtype != torch.int64 or labels.dtype != torch.int64 or (idx2 is not None and idx2.dtype != torch.int64):
+        label_rows = labels.dim() == 2   # [M, Q] floats whose argmax is the class (bio masking), else int64 [M] classes
+        if label_rows and (labels.dtype != torch.float32 or labels.shape[0] != idx.shape[0]):
+            raise PgnnError("label rows must be fp32 [M, Q] with one row per gathered row")
+        if idx.dtype != torch.int64 or not (label_rows or labels.dtype == torch.int64) or (idx2 is not None and idx2.dtype != torch.int64):
             raise PgnnError("indices and labels must be int64")
         M, D, V = idx.shape[0], rep.shape[1], w.shape[0]
         ldv = _pad4(V)  # 16-byte aligned logit rows (the tensor path's vector loads); the GEMM loaders never read past column V
@@ -929,7 +932,13 @@ class _MaskedCE(Function):
         check(lib.pgnn_linear_fwd(_p(rows), D, _p(w), _p(bias), M, V, D, 0, _p(logits), ldv, _precision, _st()), "linear_fwd")
         loss = torch.empty((), dtype=torch.float64, device=dev)
         dlogits = torch.empty(M, ldv, dtype=torch.float32, device=dev)
-        check(lib.pgnn_softmax_ce_fwd(_p(logits), ldv, M, V, _p(labels), _p(loss), _p(dlogits), ldv, _st()), "softmax_ce_fwd")
+        if label_rows:
+            wsb = int(lib.pgnn_softmax_ce_rows_workspace_bytes())
+            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+            check(lib.pgnn_softmax_ce_rows_fwd(_p(logits), ldv, M, V, _p(labels), labels.stride(0), labels.shape[1], _p(loss), _p(dlogits), ldv,
+                                               _p(ws), wsb, _st()), "softmax_ce_rows_fwd")
+        else:
+            check(lib.pgnn_softmax_ce_fwd(_p(logits), ldv, M, V, _p(labels), _p(loss), _p(dlogits), ldv, _st()), "softmax_ce_fwd")
         ctx.save_for_backward(rows, dlogits, w, idx)
         ctx.idx2 = idx2
         ctx.dims = (tuple(rep.shape), M, D, V, ldv, bias is not None)
@@ -969,3 +978,12 @@ def masked_bond_loss(node_rep, edge_index, connected_edge_indices, labels, weigh
     `edge_index[:, connected_edge_indices]`, `Linear(emb_dim, 4)`, mean CE on fp64 logits.  -> (loss fp64, logits [M, 4])."""
     me = edge_index.index_select(1, connected_edge_indices)
     return _MaskedCE.apply(node_rep, me[0], labels, weight, bias, me[1])
+
+
+def masked_edge_type_loss(node_rep, edge_index, masked_edge_idx, mask_edge_label, weight, bias=None):
+    """bio/pretrain_masking.py:47-55: `edge_rep = node_rep[u] + node_rep[v]` for the masked edges `edge_index[:, masked_edge_idx]`,
+    `Linear(emb_dim, 7)`, and CrossEntropyLoss (mean) against `torch.argmax(mask_edge_label, dim=1)`: the label of a row is the
+    first index of the maximum of its 9 label floats.  The script evaluates the loss in fp32; it is evaluated in fp64 here.
+    A label past the V classes (the maximum in column 7 or 8) raises PGNN_DEVERR_LABEL.  -> (loss fp64, logits [M, V])."""
+    me = edge_index.index_select(1, masked_edge_idx)
+    return _MaskedCE.apply(node_rep, me[0], mask_edge_label, weight, bias, me[1])

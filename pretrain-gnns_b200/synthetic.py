@@ -168,6 +168,97 @@ def ppi_batch(num_graphs: int, seed: int, n_lo: int = 400, n_hi: int = 600, pair
                 num_graphs=num_graphs)
 
 
+def ppi_graphs(batch: dict):
+    """Per-graph (num_nodes, edge_index [2,e] graph-LOCAL, edge_attr [e,9]) numpy arrays of a ppi_batch, and its edge offsets
+    [B+1] (np.int64): the form a BioDataset holds before collation."""
+    ptr = batch["ptr"].numpy()
+    ei, ea = batch["edge_index"].numpy(), batch["edge_attr"].numpy()
+    owner = np.searchsorted(ptr, ei[0], side="right") - 1  # edges are emitted graph by graph
+    eptr = np.searchsorted(owner, np.arange(len(ptr))).astype(np.int64)
+    graphs = [(int(ptr[g + 1] - ptr[g]), ei[:, eptr[g]:eptr[g + 1]] - ptr[g], ea[eptr[g]:eptr[g + 1]]) for g in range(len(ptr) - 1)]
+    return graphs, eptr
+
+
+def splitmix64(seed: int, idx) -> np.ndarray:
+    """The library's defined draw (csrc/common.cuh): the 64-bit key of each index in `idx` under `seed`, as np.uint64."""
+    with np.errstate(over="ignore"):
+        z = np.uint64(int(seed) & 0xFFFFFFFFFFFFFFFF) + (np.asarray(idx).astype(np.uint64) + np.uint64(1)) * np.uint64(0x9E3779B97F4A7C15)
+        z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        return z ^ (z >> np.uint64(31))
+
+
+def bio_masking_batch(num_graphs: int, seed: int, mask_rate: float = 0.15, one_direction: bool = False, **ppi_kw) -> dict:
+    """bio/pretrain_masking.py's input: a ppi_batch after MaskEdge (bio/util.py:46-104) and bio BatchMasking (bio/batch.py:95-96):
+    `masked_edge_idx` [M] (offset by the running edge count), `mask_edge_label` [M,9] (the edge's attribute row: multi-hot,
+    ties and all-zero rows included) and `edge_attr` with both columns of every masked pair set to [0,...,0,1].  The choice is
+    the one data.mask_edges_bio makes on the device under the same seed: per graph the int(e/2 * rate + 1) column pairs with the
+    smallest splitmix64(seed, first column) keys, ties by index.  one_direction: keep one of the two directed columns of every
+    bond first (one_direction_only); MaskEdge then masks column pairs that are two different bonds."""
+    b = ppi_batch(num_graphs, seed, **ppi_kw)
+    if one_direction:
+        b = one_direction_only(b, seed)
+    _, eoff = ppi_graphs(b)
+    idx = []
+    for g in range(num_graphs):
+        e0, m = int(eoff[g]), int(eoff[g + 1] - eoff[g]) // 2
+        k = min(int(m * mask_rate + 1), m) if m > 0 else 0      # bio/util.py:78-80
+        cols = e0 + 2 * np.arange(m, dtype=np.int64)
+        idx.append(np.sort(cols[np.lexsort((cols, splitmix64(seed, cols)))[:k]]))
+    idx = _t(np.concatenate(idx) if idx else np.zeros(0, np.int64))
+    ea = b["edge_attr"].clone()
+    b["masked_edge_idx"], b["mask_edge_label"] = idx, ea[idx].clone()
+    mask = torch.zeros(9)
+    mask[8] = 1.0                                               # bio/util.py:98-102
+    ea[idx], ea[idx + 1] = mask, mask
+    b["edge_attr"] = ea
+    return b
+
+
+def bio_context_batch(num_graphs: int, seed: int, l1: int = 1, **ppi_kw) -> dict:
+    """bio/pretrain_contextpred.py's input with the script's defaults (l1 = 1, center = 0): ExtractSubstructureContextPair
+    (bio/util.py:123-205) per ppi_batch graph and BatchSubstructContext (bio/batch.py:196-265).  The substructure side is the
+    whole ego graph and center_substruct_idx its centre node.  The context holds the nodes further than l1 hops from a root drawn
+    per graph as BioGraphStore.extract_context(center=False, seed) draws it on the device (splitmix64(seed, slot) mod n), in
+    the library's defined order: nodes ascending, the first pair of every bond (networkx keeps one edge per node pair) in
+    source order with both directions adjacent, the self-loop / mask columns zeroed (bio/loader.py:60-62), every node an
+    overlap node."""
+    from scipy.sparse import csr_matrix
+    from scipy.sparse.csgraph import shortest_path
+    b = ppi_batch(num_graphs, seed, **ppi_kw)
+    graphs, _ = ppi_graphs(b)
+    xs, eis, eas, ovs, segs, sizes, cc = [], [], [], [], [], [], 0
+    for g, (n, ei, ea) in enumerate(graphs):
+        root = int(splitmix64(seed, g) % np.uint64(n))
+        u, v = ei[0, 0::2], ei[1, 0::2]
+        first = np.zeros(len(u), bool)
+        first[np.unique(np.minimum(u, v) * n + np.maximum(u, v), return_index=True)[1]] = True
+        adj = csr_matrix((np.ones(int(first.sum())), (u[first], v[first])), shape=(n, n))
+        ctx = shortest_path(adj, directed=False, unweighted=True, indices=root) > max(int(l1), 0)
+        nc = int(ctx.sum())
+        if nc == 0:
+            raise ValueError("an ego graph has no node further than l1 = %d hops from its root" % l1)
+        new = np.cumsum(ctx) - 1
+        p = np.nonzero(first & ctx[u] & ctx[v])[0]
+        pe = np.empty((2, 2 * len(p)), np.int64)
+        pe[0, 0::2], pe[1, 0::2] = new[u[p]], new[v[p]]
+        pe[0, 1::2], pe[1, 1::2] = new[v[p]], new[u[p]]
+        pa = np.repeat(ea[2 * p], 2, axis=0)
+        pa[:, 7:] = 0
+        xs.append(np.ones((nc, 1), np.float32))
+        eis.append(pe + cc)
+        eas.append(pa)
+        ovs.append(cc + np.arange(nc, dtype=np.int64))
+        segs.append(np.full(nc, g, np.int64))
+        sizes.append(nc)
+        cc += nc
+    cat = lambda a, axis=0: np.concatenate(a, axis=axis)
+    return dict(x_substruct=b["x"], edge_index_substruct=b["edge_index"], edge_attr_substruct=b["edge_attr"],
+                center_substruct_idx=b["center_node_idx"], x_context=_t(cat(xs), torch.float32), edge_index_context=_t(cat(eis, 1)),
+                edge_attr_context=_t(cat(eas), torch.float32), overlap_context_substruct_idx=_t(cat(ovs)), batch_overlapped_context=_t(cat(segs)),
+                overlapped_context_size=_t(np.array(sizes)), num_graphs=num_graphs)
+
+
 def split_graphs(batch: dict):
     """Per-graph (x [n,2], edge_index [2,e] graph-LOCAL, edge_attr [e,2]) numpy arrays of a zinc_batch: the form a dataset
     holds before collation (chem/loader.py:53-100 builds one such Data per molecule)."""

@@ -11,6 +11,10 @@ restatement of the same bodies (oracle/steps_oracle.py) and with the reference's
     BioSupervisedStep  bio/pretrain_supervised.py:25-42   bio GNN_graphpred(5,300,T=5000), BCE on fp64 logits
     FinetuneStep       chem/finetune.py:27-46             chem GNN_graphpred(5,300,T=12) with dropout 0.5, masked BCE on fp64
                                                           logits (not a bench.py config: it is not in CONFIGS)
+    BioMaskingStep     bio/pretrain_masking.py:39-55      bio GNN(5,300,gnn_type) + Linear(300,7), CE against the argmax of the
+                                                          masked edges' label rows (not in CONFIGS)
+    BioContextPredStep bio/pretrain_contextpred.py:43-97  bio GNN(5,300) + GNN(3,300), cbow / mean pooling, BCE on fp64 scores
+                                                          (not in CONFIGS)
 """
 from __future__ import annotations
 
@@ -37,6 +41,8 @@ CONTEXT_KEYS = ("x_substruct", "edge_index_substruct", "edge_attr_substruct", "c
 BIO_KEYS = ("x", "edge_index", "edge_attr", "batch", "center_node_idx", "go_target_pretrain")
 FINETUNE_KEYS = ("x", "edge_index", "edge_attr", "batch", "y")
 FINETUNE_SEED = 5  # seed = 5 * 1000 + 1000 * rank + batch index, in the scheme of make_batches
+BIO_MASKING_KEYS = ("x", "edge_index", "edge_attr", "masked_edge_idx", "mask_edge_label")
+BIO_MASKING_SEED, BIO_CONTEXT_SEED = 6, 7
 
 
 def make_batches(config, rank, count, batch_size=None, num_tasks=5000):
@@ -119,11 +125,15 @@ class MaskingStep(_Step):
 
 class ContextPredStep(_Step):
     """chem/pretrain_contextpred.py:50-97 with the script's defaults: num_layer 5, csize 3 -> context encoder of
-    l2 - l1 = 7 - 4 = 3 layers (:145-146,156-157), mode cbow, context_pooling mean, neg_samples 1."""
-    def __init__(self, device, batch_size=128, neg_samples=1):
+    l2 - l1 = 7 - 4 = 3 layers (:145-146,156-157), mode cbow, context_pooling mean, neg_samples 1.
+    `encoder`: the GNN class of both encoders, `source(B, seed)`: the host batch of one step, drawn with seed
+    seed_base * 1000 + 1000 * rank + batch index (BioContextPredStep passes the bio ones)."""
+    def __init__(self, device, batch_size=128, neg_samples=1, encoder=chem.GNN, source=syn.substruct_context_batch,
+                 seed_base=CONFIG_ID["contextpred"]):
         self.graphs_per_batch, self.neg_samples = batch_size, neg_samples
-        self.model_substruct = chem.GNN(NUM_LAYER, EMB, JK="last", drop_ratio=0, gnn_type="gin").to(device).train()
-        self.model_context = chem.GNN(3, EMB, JK="last", drop_ratio=0, gnn_type="gin").to(device).train()
+        self.source, self.seed_base = source, seed_base
+        self.model_substruct = encoder(NUM_LAYER, EMB, JK="last", drop_ratio=0, gnn_type="gin").to(device).train()
+        self.model_context = encoder(3, EMB, JK="last", drop_ratio=0, gnn_type="gin").to(device).train()
         self.modules = [self.model_substruct, self.model_context]
         self.concurrent, self._side = True, None   # context encoder on a second CUDA stream (see scores)
         self.workload = "chem pretrain_contextpred 5-layer GIN emb_dim=300 batch_size=%d, substruct + 3-layer context encoder (BASELINE configs[2])" % batch_size
@@ -131,7 +141,7 @@ class ContextPredStep(_Step):
     KEYS = CONTEXT_KEYS
 
     def make_batches(self, rank, count):
-        return make_batches("contextpred", rank, count, self.graphs_per_batch)
+        return [_fields(self.source(self.graphs_per_batch, self.seed_base * 1000 + 1000 * rank + i), CONTEXT_KEYS) for i in range(count)]
 
     def flat_sources(self):
         return [self.model_substruct, self.model_context]
@@ -199,6 +209,50 @@ class BioSupervisedStep(_Step):
         loss = ops.bce_with_logits(pred, b["go_target_pretrain"].view(pred.shape))
         loss.backward()
         return loss
+
+
+class BioMaskingStep(_Step):
+    """bio/pretrain_masking.py:39-55 with the script's defaults (num_layer 5, emb_dim 300, dropout 0, mask_rate 0.15, batch_size 256,
+    any gnn_type): node_rep = model(x, ei, ea) on the MaskEdge'd batch; pred = linear_pred_edges(node_rep[u] + node_rep[v]) over
+    edge_index[:, masked_edge_idx]; loss = CE(pred, argmax(mask_edge_label, 1)), evaluated in fp64 (the script: fp32)."""
+    def __init__(self, device, gnn_type="gin", batch_size=256, mask_rate=0.15):
+        self.graphs_per_batch, self.mask_rate = batch_size, mask_rate
+        self.model = bio.GNN(NUM_LAYER, EMB, JK="last", drop_ratio=0, gnn_type=gnn_type).to(device).train()
+        self.head = torch.nn.Linear(EMB, 7).to(device)
+        self.modules = [self.model, self.head]
+        self.workload = ("bio pretrain_masking 5-layer %s emb_dim=300 PPI-ego-shaped graphs batch_size=%d mask_rate=%g"
+                         % (gnn_type.upper() if gnn_type != "graphsage" else "GraphSAGE", batch_size, mask_rate))
+
+    KEYS = BIO_MASKING_KEYS
+
+    def make_batches(self, rank, count):
+        return [_fields(syn.bio_masking_batch(self.graphs_per_batch, BIO_MASKING_SEED * 1000 + 1000 * rank + i, self.mask_rate), BIO_MASKING_KEYS)
+                for i in range(count)]
+
+    def flat_sources(self):
+        return [self.model]
+
+    def named_modules(self):
+        return {"model": self.model, "head": self.head}
+
+    def __call__(self, b):
+        self.zero_grad()
+        rep = self.model(b["x"], b["edge_index"], b["edge_attr"])
+        loss, _ = ops.masked_edge_type_loss(rep, b["edge_index"], b["masked_edge_idx"], b["mask_edge_label"], self.head.weight, self.head.bias)
+        loss.backward()
+        return loss
+
+
+class BioContextPredStep(ContextPredStep):
+    """bio/pretrain_contextpred.py:43-97 with the script's defaults (num_layer 5, emb_dim 300, batch_size 256, l1 1, center 0, mode
+    cbow, context_pooling mean, neg_samples 1): bio GNN(5, 300) over the whole ego graphs read at their centre nodes, bio
+    GNN(3, 300) over the context (the nodes further than l1 hops from a random root), then ContextPredStep's head."""
+    def __init__(self, device, batch_size=256, neg_samples=1, l1=1):
+        super().__init__(device, batch_size, neg_samples, encoder=bio.GNN, source=lambda B, seed: syn.bio_context_batch(B, seed, l1),
+                         seed_base=BIO_CONTEXT_SEED)
+        self.l1 = l1
+        self.workload = ("bio pretrain_contextpred 5-layer GIN emb_dim=300 PPI-ego-shaped graphs batch_size=%d l1=%d, substruct + 3-layer "
+                         "context encoder" % (batch_size, l1))
 
 
 class FinetuneStep(_Step):
