@@ -126,7 +126,7 @@ PGNN_API int pgnn_bio_embed_bwd(const float* x, const float* g, int64_t ldg, int
  *   out[i, 0:C]           = sum_k w_k * x[nbr_t[k], 0:C] + w_ii * x[i, 0:C]   (+ S[i,:] . T if edge_off == 0)
  *   out[i, edge_off: +C]  = S[i,:] . T                                       (if edge_off > 0: bio GIN concat,
  *                                                                              bio/model.py:54-55)
- * x may be given as (pre-BN activations, per-column affine, ReLU flag): x_eff = act(x * in_scale + in_shift)
+ * x may be given as (pre-BN activations, per-column affine, ReLU flag): x_eff = act(fmaf(x, in_scale, in_shift))
  * so a BatchNorm + ReLU (chem/model.py:269-275) is applied on load instead of in a pass of its own
  * (in_scale == NULL -> identity).  The ReLU keeps NaN, as torch.relu does.
  * ------------------------------------------------------------------------------------------- */
@@ -166,10 +166,11 @@ PGNN_API int pgnn_linear_bwd_w(const float* gy, int64_t ldgy, const float* x, in
  * Statistics are accumulated in fp64 (block partials folded with fp64 atomics: order effects ~1e-16).
  * ------------------------------------------------------------------------------------------- */
 PGNN_API int64_t pgnn_bn_workspace_bytes(int64_t M, int64_t C);
-/* train: batch statistics (biased var), y = act((x-mean)*invstd*gamma+beta); save_mean/save_invstd [C]
- * written for backward; running_mean/var (unbiased var) and *num_batches_tracked updated in place
- * when non-NULL.  y may be NULL (statistics only: the consumer applies scale/shift on load);
- * scale/shift [C] (y = x*scale + shift) are written when non-NULL. */
+/* train: batch statistics (biased var), y = act(fmaf(x, scale, shift)) with scale = gamma*invstd and
+ * shift = fmaf(-mean, scale, beta) (fp32, one rounding each); save_mean/save_invstd [C] written for backward;
+ * running_mean/var (unbiased var) and *num_batches_tracked updated in place when non-NULL.  y may be NULL
+ * (statistics only: the consumer applies scale/shift on load); scale/shift [C] are written when non-NULL.
+ * Any 0 < M < 2^31. */
 PGNN_API int pgnn_bn_fwd_train(const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma,
                                const float* beta, float* running_mean, float* running_var,
                                int64_t* num_batches_tracked, float momentum, float eps, int relu,
@@ -180,7 +181,7 @@ PGNN_API int pgnn_bn_fwd_eval(const float* x, int64_t ldx, int64_t M, int64_t C,
                               const float* beta, const float* running_mean, const float* running_var,
                               float eps, int relu, float* y, int64_t ldy, void* stream);
 /* gx = BN'(gy * relu_mask); ggamma/gbeta [C] OVERWRITTEN.  relu != 0: mask = (y > 0) with y recomputed
- * from x, save_mean, save_invstd, gamma, beta. */
+ * bit for bit from x, save_mean, save_invstd, gamma, beta by the forward's expression above. */
 PGNN_API int pgnn_bn_bwd(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t C,
                          const float* gamma, const float* beta, const float* save_mean,
                          const float* save_invstd, int relu, float* gx, int64_t ldgx, float* ggamma,
@@ -305,6 +306,9 @@ PGNN_API int64_t pgnn_chem_gin_workspace_bytes(int64_t N, int64_t E, int64_t L, 
 /* test aid: byte offsets in the workspace of z1 [L][N][2D] (post-ReLU hidden), z2 [L][N][D] (pre-BatchNorm), BatchNorm batch mean
  * [L][D] and invstd [L][D] after a training forward: lets a test recover the ReLU decisions the encoder took */
 PGNN_API int pgnn_chem_gin_debug_layout(int64_t N, int64_t E, int64_t L, int64_t D, int64_t* out4);
+/* test aid: byte offset in the same workspace of aggr [L][N][D], layer l's gathered input after a training forward (for l > 0 the
+ * previous layer's BatchNorm + ReLU as the gather applied it on load); PGNN_EINVAL for bad sizes */
+PGNN_API int64_t pgnn_chem_gin_debug_aggr_offset(int64_t N, int64_t E, int64_t L, int64_t D);
 /* test aids for the 3xTF32 wgmma GEMM (precision 1), reachable here with every operand layout, tile width and epilogue:
  *   pgnn_debug_tc_gemm: C[m,n] = sum_r A(m,r) B(n,r), r < K.  a_kc / b_kc != 0: the operand is reduction-contiguous
  *     (A(m,r) = A[m*lda + r]), else A(m,r) = A[r*lda + m] (same for B with n).  bn = the tile width, 64 or 128.  Epilogue as in
@@ -327,6 +331,22 @@ PGNN_API int pgnn_debug_tc_wgrad(const float* gy, int64_t ldgy, const float* x, 
 PGNN_API int pgnn_debug_tc_wgrad_plan(int64_t M, int64_t N, int64_t K, int64_t* out4);
 PGNN_API int pgnn_debug_transpose_batch(int count, const float* const* in, float* const* out, const int32_t* rows,
                                         const int32_t* cols, void* stream);
+/* test aids for the two BatchNorm sweeps only the whole encoder reaches (dropout of (drop_p, drop_seed, drop_layer) as in
+ * pgnn_dropout_fwd; drop_p = 0 runs the mask-free kernels):
+ *   pgnn_debug_bn_apply_fold: pgnn_bn_fwd_train's finalisation and apply in one kernel, from raw fp64 sums[2][C] (sum, sum of
+ *     squares of the M rows of x).  Every CTA derives scale / shift itself (invstd = 1 / sqrtf((float)var + eps)); CTA 0 alone
+ *     writes save_mean / save_invstd and updates running_mean / running_var / *num_batches_tracked (each may be NULL).
+ *     C <= 6144 (scale / shift live in 48 KiB of shared memory).
+ *   pgnn_debug_bn_bwd_colsum: pgnn_bn_bwd (mask applied to gy before the ReLU mask) that also leaves the column sums of gx in
+ *     colsum[C] (OVERWRITTEN).  Row strides ldgy, ldx, ldgx >= C. */
+PGNN_API int pgnn_debug_bn_apply_fold(const float* x, int64_t ldx, int64_t M, int64_t C, const double* sums, const float* gamma,
+                                      const float* beta, float* running_mean, float* running_var, int64_t* num_batches_tracked,
+                                      float momentum, float eps, float* save_mean, float* save_invstd, int relu, float* y, int64_t ldy,
+                                      float drop_p, int64_t drop_seed, int64_t drop_layer, void* stream);
+PGNN_API int pgnn_debug_bn_bwd_colsum(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t C,
+                                      const float* gamma, const float* beta, const float* save_mean, const float* save_invstd, int relu,
+                                      float* gx, int64_t ldgx, float* ggamma, float* gbeta, float* colsum, float drop_p,
+                                      int64_t drop_seed, int64_t drop_layer, void* workspace, int64_t workspace_bytes, void* stream);
 PGNN_API int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
                                    void* const* bn_num_batches_tracked, const int64_t* x, const int64_t* edge_index,
                                    const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, int training,

@@ -20,10 +20,10 @@ __device__ __forceinline__ float4 affine_act(float4 v, const float* __restrict__
                                              int c, int relu) {
   if (sc) {
     const float4 a = ld4(sc + c), b = ld4(sh + c);
-    v.x = fmaf(v.x, a.x, b.x);
-    v.y = fmaf(v.y, a.y, b.y);
-    v.z = fmaf(v.z, a.z, b.z);
-    v.w = fmaf(v.w, a.w, b.w);
+    v.x = bn_preact(v.x, a.x, b.x);  // the BatchNorm pre-activation of common.cuh: the backward recomputes it bit for bit
+    v.y = bn_preact(v.y, a.y, b.y);
+    v.z = bn_preact(v.z, a.z, b.z);
+    v.w = bn_preact(v.w, a.w, b.w);
   }
   if (relu) {
     v.x = relu_keep_nan(v.x);

@@ -77,6 +77,18 @@ struct PgnnBnFold {
   }
 };
 
+// The BatchNorm pre-activation, defined once: y = act(fmaf(x, scale, shift)) with scale = gamma * invstd and
+// shift = fmaf(-mean, scale, beta), all in fp32 with one rounding each.  Every forward apply (norm.cu, and the gathers of
+// aggregate.cu that apply the previous layer's BatchNorm + ReLU on load) computes this expression, and every backward sweep
+// recomputes it bit for bit from save_mean / save_invstd / gamma / beta: the ReLU mask of the backward is the decision the
+// forward took.  (Two differently rounded expressions, e.g. fmaf((x - mean) * invstd, gamma, beta), disagree in sign for
+// pre-activations within a few ulps of zero, and the gradient of such an element is then off by a whole gy entry.)
+__device__ __forceinline__ float bn_scale(float gamma, float invstd) { return __fmul_rn(gamma, invstd); }
+__device__ __forceinline__ float bn_shift(float mean, float scale, float beta) { return __fmaf_rn(-mean, scale, beta); }
+__device__ __forceinline__ float bn_preact(float x, float scale, float shift) { return __fmaf_rn(x, scale, shift); }
+// the backward's ReLU test: the gradient passes iff the forward's output was > 0 (a NaN or +-0 output passes none)
+__device__ __forceinline__ bool bn_relu_keep(float x, float scale, float shift) { return bn_preact(x, scale, shift) > 0.f; }
+
 // per-column BatchNorm constants from the accumulated sums; `leader` performs the running-statistics side effects
 // Every CTA of the consumer runs this for its columns, so it must be cheap: the fp64 part is two multiplies and one FMA (the
 // sums are fp64 because E[x^2] - E[x]^2 cancels); the reciprocal square root is taken in fp32 like torch's own BatchNorm
@@ -89,8 +101,8 @@ __device__ __forceinline__ void bn_fold_column(const PgnnBnFold& f, int C, int c
   var = var < 0.0 ? 0.0 : var;
   const float invstd = 1.0f / sqrtf((float)var + f.eps);
   const float meanf = (float)mean;
-  scale = f.gamma[c] * invstd;
-  shift = fmaf(-meanf, scale, f.beta[c]);
+  scale = bn_scale(f.gamma[c], invstd);
+  shift = bn_shift(meanf, scale, f.beta[c]);
   if (leader) {
     if (f.save_mean) f.save_mean[c] = meanf;
     if (f.save_invstd) f.save_invstd[c] = invstd;

@@ -700,6 +700,15 @@ int pgnn_chem_gin_debug_layout(int64_t N, int64_t E, int64_t L, int64_t D, int64
   return PGNN_OK;
 }
 
+// Test aid: byte offset inside the workspace of aggr ([L][N][D]): layer l's gathered input, i.e. for l > 0 the previous layer's
+// BatchNorm + ReLU as the gather applied it on load (with no edges and zero edge tables, exactly act(z2[l-1]) row for row)
+int64_t pgnn_chem_gin_debug_aggr_offset(int64_t N, int64_t E, int64_t L, int64_t D) {
+  if (N < 0 || E < 0 || L < 1 || D <= 0) return PGNN_EINVAL;
+  char* base = reinterpret_cast<char*>(0x1000);
+  GinWs w = carve_gin(base, N, E, L, D);
+  return reinterpret_cast<char*>(w.aggr) - base;
+}
+
 // ------------------------------------------------------------------------------------------------------------------------------
 // GCN / GraphSAGE / GAT
 // ------------------------------------------------------------------------------------------------------------------------------

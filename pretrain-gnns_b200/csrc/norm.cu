@@ -23,6 +23,14 @@ inline bool bn_v4_enabled() {
 }
 
 constexpr int kStatRows = 128;  // rows per block of the statistics sweeps
+// The row sweeps launch one block row per chunk of rows, at most kMaxGridY of them (the limit of gridDim.y): block row y
+// handles chunks y, y + gridDim.y, ... in that order, so the fold below has the same structure at every M, and any M < 2^31
+// is computed rather than refused at launch.
+constexpr int64_t kMaxGridY = 65535;
+inline unsigned row_blocks(int64_t M, int rows) {
+  const int64_t b = ceil_div(M, rows);
+  return (unsigned)(b < kMaxGridY ? b : kMaxGridY);
+}
 
 // sums of f0(row, col) and f1(row, col) over the rows, per column -> acc[0][C], acc[1][C] (fp64 atomics)
 template <typename F>
@@ -30,15 +38,17 @@ __device__ __forceinline__ void column_pair_sums(int M, int C, double* __restric
   __shared__ double red[2][8][33];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int c = blockIdx.x * 32 + lane;
-  const int r0 = blockIdx.y * kStatRows, r1 = min(M, r0 + kStatRows);
   double s0 = 0.0, s1 = 0.0;
   if (c < C) {
+    for (unsigned r0 = blockIdx.y * kStatRows; r0 < (unsigned)M; r0 += gridDim.y * kStatRows) {
+      const int r1 = (int)min((unsigned)M, r0 + kStatRows);
 #pragma unroll 4
-    for (int r = r0 + w; r < r1; r += 8) {
-      double a, b;
-      f(r, c, a, b);
-      s0 += a;
-      s1 += b;
+      for (int r = (int)r0 + w; r < r1; r += 8) {
+        double a, b;
+        f(r, c, a, b);
+        s0 += a;
+        s1 += b;
+      }
     }
   }
   red[0][w][lane] = s0;
@@ -85,9 +95,9 @@ k_bn_finalize(const double* __restrict__ acc, int M, int C, const float* __restr
     running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)unbiased;
   }
   if (scale) {
-    const float sc = gamma[c] * invstd;
+    const float sc = bn_scale(gamma[c], invstd);
     scale[c] = sc;
-    shift[c] = fmaf(-meanf, sc, beta[c]);
+    shift[c] = bn_shift(meanf, sc, beta[c]);
   }
 }
 
@@ -104,7 +114,8 @@ __device__ __forceinline__ void bn_apply_body(const float* __restrict__ x, int64
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = idx / C;
     const int c = (int)(idx - r * C);
-    float v = fmaf((x[r * ldx + c] - mean[c]) * invstd[c], gamma[c], beta[c]);
+    const float sc = bn_scale(gamma[c], invstd[c]);
+    float v = bn_preact(x[r * ldx + c], sc, bn_shift(mean[c], sc, beta[c]));
     if (relu) v = relu_keep_nan(v);
     if (DROP) v *= dropout_factor(drop, r, C, c);
     y[r * ldy + c] = v;
@@ -135,7 +146,7 @@ __device__ __forceinline__ void bn_apply_fold_body(const float* __restrict__ x, 
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = idx / C;
     const int c = (int)(idx - r * C);
-    float v = fmaf(x[r * ldx + c], s_aff[c], s_aff[C + c]);
+    float v = bn_preact(x[r * ldx + c], s_aff[c], s_aff[C + c]);
     if (relu) v = relu_keep_nan(v);
     if (DROP) v *= dropout_factor(drop, r, C, c);
     y[r * ldy + c] = v;
@@ -174,11 +185,21 @@ __device__ __forceinline__ void bn_bwd_stats_body(const float* __restrict__ gy, 
                                                   const float* __restrict__ mean, const float* __restrict__ invstd, int relu,
                                                   double* __restrict__ acc, const PgnnDropout& drop) {
   pdl_prologue();
+  // a thread sums one column (column_pair_sums' c): its BatchNorm constants are loaded and derived once, not per row
+  const int cc = blockIdx.x * 32 + (threadIdx.x & 31);
+  float mu = 0.f, is = 0.f, sc = 0.f, sh = 0.f;
+  if (cc < C) {
+    mu = mean[cc];
+    is = invstd[cc];
+    sc = bn_scale(gamma[cc], is);
+    sh = bn_shift(mu, sc, beta[cc]);
+  }
   column_pair_sums(M, C, acc, [&](int r, int c, double& a, double& b) {
-    const float xhat = (x[(int64_t)r * ldx + c] - mean[c]) * invstd[c];
+    const float xv = x[(int64_t)r * ldx + c];
+    const float xhat = (xv - mu) * is;
     float d = gy[(int64_t)r * ldgy + c];
     if (DROP) d *= dropout_factor(drop, r, C, c);
-    if (relu && !(fmaf(xhat, gamma[c], beta[c]) > 0.f)) d = 0.f;
+    if (relu && !bn_relu_keep(xv, sc, sh)) d = 0.f;
     a = (double)d;
     b = (double)d * (double)xhat;  // exact product: small batches make the BN backward a difference of large terms
   });
@@ -220,10 +241,14 @@ __device__ __forceinline__ void bn_bwd_apply_body(const float* __restrict__ gy, 
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = idx / C;
     const int c = (int)(idx - r * C);
-    const float xhat = (x[r * ldx + c] - mean[c]) * invstd[c];
+    const float xv = x[r * ldx + c];
+    const float xhat = (xv - mean[c]) * invstd[c];
     float d = gy[r * ldgy + c];
     if (DROP) d *= dropout_factor(drop, r, C, c);
-    if (relu && !(fmaf(xhat, gamma[c], beta[c]) > 0.f)) d = 0.f;
+    if (relu) {
+      const float sc = bn_scale(gamma[c], invstd[c]);
+      if (!bn_relu_keep(xv, sc, bn_shift(mean[c], sc, beta[c]))) d = 0.f;
+    }
     gx[r * ldgx + c] = gamma[c] * invstd[c] * (d - c1[c] - xhat * c2[c]);
   }
 }
@@ -255,7 +280,6 @@ __device__ __forceinline__ void bn_bwd_apply_colsum_body(const float* __restrict
   __shared__ float red[8][33];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int c = blockIdx.x * 32 + lane;
-  const int r0 = blockIdx.y * kStatRows, r1 = min(M, r0 + kStatRows);
   float acc = 0.f;
   if (c < C) {
     // finalisation of the statistics pass folded in: sum(dy), sum(dy*xhat) -> the two BatchNorm-backward means
@@ -264,16 +288,21 @@ __device__ __forceinline__ void bn_bwd_apply_colsum_body(const float* __restrict
       if (gbeta) gbeta[c] = (float)sd;
       if (ggamma) ggamma[c] = (float)sdx;
     }
-    const float mu = mean[c], is = invstd[c], ga = gamma[c], be = beta[c], k1 = (float)(sd / M), k2 = (float)(sdx / M);
+    const float mu = mean[c], is = invstd[c], ga = gamma[c], k1 = (float)(sd / M), k2 = (float)(sdx / M);
+    const float sc = bn_scale(ga, is), sh = bn_shift(mu, sc, beta[c]);
+    for (unsigned r0 = blockIdx.y * kStatRows; r0 < (unsigned)M; r0 += gridDim.y * kStatRows) {
+      const int r1 = (int)min((unsigned)M, r0 + kStatRows);
 #pragma unroll 4
-    for (int r = r0 + w; r < r1; r += 8) {
-      const float xhat = (x[(int64_t)r * ldx + c] - mu) * is;
-      float d = gy[(int64_t)r * ldgy + c];
-      if (DROP) d *= dropout_factor(drop, r, C, c);
-      if (relu && !(fmaf(xhat, ga, be) > 0.f)) d = 0.f;
-      const float v = ga * is * (d - k1 - xhat * k2);
-      gx[(int64_t)r * ldgx + c] = v;
-      acc += v;
+      for (int r = (int)r0 + w; r < r1; r += 8) {
+        const float xv = x[(int64_t)r * ldx + c];
+        const float xhat = (xv - mu) * is;
+        float d = gy[(int64_t)r * ldgy + c];
+        if (DROP) d *= dropout_factor(drop, r, C, c);
+        if (relu && !bn_relu_keep(xv, sc, sh)) d = 0.f;
+        const float v = ga * is * (d - k1 - xhat * k2);
+        gx[(int64_t)r * ldgx + c] = v;
+        acc += v;
+      }
     }
   }
   red[w][lane] = acc;
@@ -319,24 +348,28 @@ __device__ __forceinline__ void bn_bwd_stats_v4_body(const float* __restrict__ g
   __shared__ double red[2][8][128];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int c = blockIdx.x * 128 + lane * 4;
-  const int r0 = blockIdx.y * kVecRows, r1 = min(M, r0 + kVecRows);
   double s0[4] = {0.0, 0.0, 0.0, 0.0}, s1[4] = {0.0, 0.0, 0.0, 0.0};
   if (c < C) {
     const float4 mu = ldg4(mean + c), is = ldg4(invstd + c), ga = ldg4(gamma + c), be = ldg4(beta + c);
-    const float muv[4] = {mu.x, mu.y, mu.z, mu.w}, isv[4] = {is.x, is.y, is.z, is.w}, gav[4] = {ga.x, ga.y, ga.z, ga.w},
-                bev[4] = {be.x, be.y, be.z, be.w};
+    const float muv[4] = {mu.x, mu.y, mu.z, mu.w}, isv[4] = {is.x, is.y, is.z, is.w}, bev[4] = {be.x, be.y, be.z, be.w};
+    const float scv[4] = {bn_scale(ga.x, is.x), bn_scale(ga.y, is.y), bn_scale(ga.z, is.z), bn_scale(ga.w, is.w)};
+    const float shv[4] = {bn_shift(muv[0], scv[0], bev[0]), bn_shift(muv[1], scv[1], bev[1]), bn_shift(muv[2], scv[2], bev[2]),
+                          bn_shift(muv[3], scv[3], bev[3])};
+    for (unsigned r0 = blockIdx.y * kVecRows; r0 < (unsigned)M; r0 += gridDim.y * kVecRows) {
+      const int r1 = (int)min((unsigned)M, r0 + kVecRows);
 #pragma unroll 4
-    for (int r = r0 + w; r < r1; r += 8) {
-      const float4 xv = ldg4(x + (int64_t)r * ldx + c), gv = ldg4(gy + (int64_t)r * ldgy + c);
-      const float xs[4] = {xv.x, xv.y, xv.z, xv.w}, gs[4] = {gv.x, gv.y, gv.z, gv.w};
+      for (int r = (int)r0 + w; r < r1; r += 8) {
+        const float4 xv = ldg4(x + (int64_t)r * ldx + c), gv = ldg4(gy + (int64_t)r * ldgy + c);
+        const float xs[4] = {xv.x, xv.y, xv.z, xv.w}, gs[4] = {gv.x, gv.y, gv.z, gv.w};
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float xhat = (xs[q] - muv[q]) * isv[q];
-        float d = gs[q];
-        if (DROP) d *= dropout_factor(drop, r, C, c + q);
-        if (relu && !(fmaf(xhat, gav[q], bev[q]) > 0.f)) d = 0.f;
-        s0[q] += (double)d;
-        s1[q] += (double)d * (double)xhat;
+        for (int q = 0; q < 4; ++q) {
+          const float xhat = (xs[q] - muv[q]) * isv[q];
+          float d = gs[q];
+          if (DROP) d *= dropout_factor(drop, r, C, c + q);
+          if (relu && !bn_relu_keep(xs[q], scv[q], shv[q])) d = 0.f;
+          s0[q] += (double)d;
+          s1[q] += (double)d * (double)xhat;
+        }
       }
     }
   }
@@ -379,12 +412,14 @@ __device__ __forceinline__ void bn_bwd_apply_colsum_v4_body(const float* __restr
   __shared__ float red[8][128];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int c = blockIdx.x * 128 + lane * 4;
-  const int r0 = blockIdx.y * kVecRows, r1 = min(M, r0 + kVecRows);
   float acc[4] = {0.f, 0.f, 0.f, 0.f};
   if (c < C) {
     const float4 mu = ldg4(mean + c), is = ldg4(invstd + c), ga = ldg4(gamma + c), be = ldg4(beta + c);
     const float muv[4] = {mu.x, mu.y, mu.z, mu.w}, isv[4] = {is.x, is.y, is.z, is.w}, gav[4] = {ga.x, ga.y, ga.z, ga.w},
                 bev[4] = {be.x, be.y, be.z, be.w};
+    const float scv[4] = {bn_scale(gav[0], isv[0]), bn_scale(gav[1], isv[1]), bn_scale(gav[2], isv[2]), bn_scale(gav[3], isv[3])};
+    const float shv[4] = {bn_shift(muv[0], scv[0], bev[0]), bn_shift(muv[1], scv[1], bev[1]), bn_shift(muv[2], scv[2], bev[2]),
+                          bn_shift(muv[3], scv[3], bev[3])};
     float k1[4], k2[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
@@ -396,21 +431,24 @@ __device__ __forceinline__ void bn_bwd_apply_colsum_v4_body(const float* __restr
         if (ggamma) ggamma[c + q] = (float)sdx;
       }
     }
+    for (unsigned r0 = blockIdx.y * kVecRows; r0 < (unsigned)M; r0 += gridDim.y * kVecRows) {
+      const int r1 = (int)min((unsigned)M, r0 + kVecRows);
 #pragma unroll 4
-    for (int r = r0 + w; r < r1; r += 8) {
-      const float4 xv = ldg4(x + (int64_t)r * ldx + c), gv = ldg4(gy + (int64_t)r * ldgy + c);
-      const float xs[4] = {xv.x, xv.y, xv.z, xv.w}, gs[4] = {gv.x, gv.y, gv.z, gv.w};
-      float o[4];
+      for (int r = (int)r0 + w; r < r1; r += 8) {
+        const float4 xv = ldg4(x + (int64_t)r * ldx + c), gv = ldg4(gy + (int64_t)r * ldgy + c);
+        const float xs[4] = {xv.x, xv.y, xv.z, xv.w}, gs[4] = {gv.x, gv.y, gv.z, gv.w};
+        float o[4];
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float xhat = (xs[q] - muv[q]) * isv[q];
-        float d = gs[q];
-        if (DROP) d *= dropout_factor(drop, r, C, c + q);
-        if (relu && !(fmaf(xhat, gav[q], bev[q]) > 0.f)) d = 0.f;
-        o[q] = gav[q] * isv[q] * (d - k1[q] - xhat * k2[q]);
-        acc[q] += o[q];
+        for (int q = 0; q < 4; ++q) {
+          const float xhat = (xs[q] - muv[q]) * isv[q];
+          float d = gs[q];
+          if (DROP) d *= dropout_factor(drop, r, C, c + q);
+          if (relu && !bn_relu_keep(xs[q], scv[q], shv[q])) d = 0.f;
+          o[q] = gav[q] * isv[q] * (d - k1[q] - xhat * k2[q]);
+          acc[q] += o[q];
+        }
+        *reinterpret_cast<float4*>(gx + (int64_t)r * ldgx + c) = make_float4(o[0], o[1], o[2], o[3]);
       }
-      *reinterpret_cast<float4*>(gx + (int64_t)r * ldgx + c) = make_float4(o[0], o[1], o[2], o[3]);
     }
   }
 #pragma unroll
@@ -423,7 +461,8 @@ __device__ __forceinline__ void bn_bwd_apply_colsum_v4_body(const float* __restr
     atomicAdd(&colsum[blockIdx.x * 128 + threadIdx.x], t);
   }
 }
-__global__ void __launch_bounds__(256)
+// (three CTAs per SM, as before the ReLU test recomputed scale / shift: 80 registers, no spills)
+__global__ void __launch_bounds__(256, 3)
 k_bn_bwd_apply_colsum_v4(const float* __restrict__ gy, int64_t ldgy, const float* __restrict__ x, int64_t ldx, int M, int C,
                          const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ mean,
                          const float* __restrict__ invstd, int relu, const double* __restrict__ sums, float* __restrict__ ggamma,
@@ -448,17 +487,19 @@ k_bn_stats_v4(const float* __restrict__ x, int64_t ldx, int M, int C, double* __
   __shared__ double red[2][8][128];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int c = blockIdx.x * 128 + lane * 4;
-  const int r0 = blockIdx.y * kVecRows, r1 = min(M, r0 + kVecRows);
   double s0[4] = {0.0, 0.0, 0.0, 0.0}, s1[4] = {0.0, 0.0, 0.0, 0.0};
   if (c < C) {
+    for (unsigned r0 = blockIdx.y * kVecRows; r0 < (unsigned)M; r0 += gridDim.y * kVecRows) {
+      const int r1 = (int)min((unsigned)M, r0 + kVecRows);
 #pragma unroll 8
-    for (int r = r0 + w; r < r1; r += 8) {
-      const float4 xv = ldg4(x + (int64_t)r * ldx + c);
-      const double v[4] = {(double)xv.x, (double)xv.y, (double)xv.z, (double)xv.w};
+      for (int r = (int)r0 + w; r < r1; r += 8) {
+        const float4 xv = ldg4(x + (int64_t)r * ldx + c);
+        const double v[4] = {(double)xv.x, (double)xv.y, (double)xv.z, (double)xv.w};
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        s0[q] += v[q];
-        s1[q] += v[q] * v[q];
+        for (int q = 0; q < 4; ++q) {
+          s0[q] += v[q];
+          s1[q] += v[q] * v[q];
+        }
       }
     }
   }
@@ -488,11 +529,12 @@ __device__ __forceinline__ void bn_apply_v4_body(const float* __restrict__ x, in
     const int64_t r = idx / C4;
     const int c = (int)(idx - r * C4) * 4;
     const float4 xv = ldg4(x + r * ldx + c), mu = ldg4(mean + c), is = ldg4(invstd + c), ga = ldg4(gamma + c), be = ldg4(beta + c);
+    const float4 sc = make_float4(bn_scale(ga.x, is.x), bn_scale(ga.y, is.y), bn_scale(ga.z, is.z), bn_scale(ga.w, is.w));
     float4 o;
-    o.x = fmaf((xv.x - mu.x) * is.x, ga.x, be.x);
-    o.y = fmaf((xv.y - mu.y) * is.y, ga.y, be.y);
-    o.z = fmaf((xv.z - mu.z) * is.z, ga.z, be.z);
-    o.w = fmaf((xv.w - mu.w) * is.w, ga.w, be.w);
+    o.x = bn_preact(xv.x, sc.x, bn_shift(mu.x, sc.x, be.x));
+    o.y = bn_preact(xv.y, sc.y, bn_shift(mu.y, sc.y, be.y));
+    o.z = bn_preact(xv.z, sc.z, bn_shift(mu.z, sc.z, be.z));
+    o.w = bn_preact(xv.w, sc.w, bn_shift(mu.w, sc.w, be.w));
     if (relu) {
       o.x = relu_keep_nan(o.x); o.y = relu_keep_nan(o.y); o.z = relu_keep_nan(o.z); o.w = relu_keep_nan(o.w);
     }
@@ -638,7 +680,7 @@ int pgnn_internal_bn_bwd_colsum(const float* gy, int64_t ldgy, const float* x, i
   auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
   if (bn_v4_enabled() && C % 4 == 0 && ldgy % 4 == 0 && ldx % 4 == 0 && ldgx % 4 == 0 && a16(gy) && a16(x) && a16(gx) && a16(gamma) && a16(beta) &&
       a16(save_mean) && a16(save_invstd)) {
-    dim3 gv((unsigned)ceil_div(C, 128), (unsigned)ceil_div(M, kVecRows));
+    dim3 gv((unsigned)ceil_div(C, 128), row_blocks(M, kVecRows));
     if (dr)
       PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_v4_drop, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd,
                             relu, acc, *dr));
@@ -654,7 +696,7 @@ int pgnn_internal_bn_bwd_colsum(const float* gy, int64_t ldgy, const float* x, i
     PGNN_LAUNCH_CHECK();
     return PGNN_OK;
   }
-  dim3 g1((unsigned)ceil_div(C, 32), (unsigned)ceil_div(M, kStatRows));
+  dim3 g1((unsigned)ceil_div(C, 32), row_blocks(M, kStatRows));
   if (dr)
     PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_drop, dim3(g1), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu,
                           acc, *dr));
@@ -687,10 +729,10 @@ int pgnn_internal_bn_fwd_train(const float* x, int64_t ldx, int64_t M, int64_t C
   const bool v4 = bn_v4_enabled() && C % 4 == 0 && ldx % 4 == 0 && a16(x) && a16(gamma) && a16(beta) && a16(save_mean) && a16(save_invstd) &&
                   (!y || (ldy % 4 == 0 && a16(y)));
   if (v4) {
-    dim3 gv((unsigned)ceil_div(C, 128), (unsigned)ceil_div(M, kVecRows));
+    dim3 gv((unsigned)ceil_div(C, 128), row_blocks(M, kVecRows));
     PGNN_CUDA(pgnn_launch(k_bn_stats_v4, dim3(gv), dim3(256), 0, st, x, ldx, (int)M, (int)C, acc));
   } else {
-    dim3 g1((unsigned)ceil_div(C, 32), (unsigned)ceil_div(M, kStatRows));
+    dim3 g1((unsigned)ceil_div(C, 32), row_blocks(M, kStatRows));
     PGNN_CUDA(pgnn_launch(k_bn_stats, dim3(g1), dim3(256), 0, st, x, ldx, (int)M, (int)C, acc));
   }
   PGNN_LAUNCH_CHECK();
@@ -728,7 +770,7 @@ int pgnn_internal_bn_bwd(const float* gy, int64_t ldgy, const float* x, int64_t 
     auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
     if (bn_v4_enabled() && C % 4 == 0 && ldgy % 4 == 0 && ldx % 4 == 0 && ldgx % 4 == 0 && a16(gy) && a16(x) && a16(gx) && a16(gamma) && a16(beta) &&
         a16(save_mean) && a16(save_invstd)) {
-      dim3 gv((unsigned)ceil_div(C, 128), (unsigned)ceil_div(M, kVecRows));
+      dim3 gv((unsigned)ceil_div(C, 128), row_blocks(M, kVecRows));
       if (dr)
         PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_v4_drop, dim3(gv), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd,
                               relu, acc, *dr));
@@ -745,7 +787,7 @@ int pgnn_internal_bn_bwd(const float* gy, int64_t ldgy, const float* x, int64_t 
       return PGNN_OK;
     }
   }
-  dim3 g1((unsigned)ceil_div(C, 32), (unsigned)ceil_div(M, kStatRows));
+  dim3 g1((unsigned)ceil_div(C, 32), row_blocks(M, kStatRows));
   if (dr)
     PGNN_CUDA(pgnn_launch(k_bn_bwd_stats_drop, dim3(g1), dim3(256), 0, st, gy, ldgy, x, ldx, (int)M, (int)C, gamma, beta, save_mean, save_invstd, relu,
                           acc, *dr));
@@ -845,6 +887,34 @@ int pgnn_l2norm_bwd(const float* gy, int64_t ldgy, const float* y, int64_t ldy_,
   PGNN_CUDA(pgnn_launch(k_l2norm_bwd, dim3(grid_items(M * 32, 256)), dim3(256), 0, as_stream(stream), gy, ldgy, y, ldy_, norm, M, (int)C, gx, ldgx));
   PGNN_LAUNCH_CHECK();
   return PGNN_OK;
+}
+
+int pgnn_debug_bn_apply_fold(const float* x, int64_t ldx, int64_t M, int64_t C, const double* sums, const float* gamma, const float* beta,
+                             float* running_mean, float* running_var, int64_t* num_batches_tracked, float momentum, float eps,
+                             float* save_mean, float* save_invstd, int relu, float* y, int64_t ldy, float drop_p, int64_t drop_seed,
+                             int64_t drop_layer, void* stream) {
+  PGNN_CHECK_ARG(M > 0 && C > 0 && M < (1ll << 31) && C <= 6144 && x && sums && gamma && beta && y && ldx >= C && ldy >= C);
+  PgnnDropout drop;
+  PGNN_CHECK_ARG(pgnn_make_dropout(drop_p, drop_seed, drop_layer, &drop));
+  PgnnBnFold fold;
+  fold.acc = sums; fold.gamma = gamma; fold.beta = beta;
+  fold.running_mean = running_mean; fold.running_var = running_var; fold.nbt = num_batches_tracked;
+  fold.save_mean = save_mean; fold.save_invstd = save_invstd;
+  fold.momentum = momentum; fold.eps = eps; fold.set_rows((int)M);
+  return pgnn_internal_bn_apply_fold(x, ldx, M, C, fold, relu, y, ldy, as_stream(stream), &drop);
+}
+
+int pgnn_debug_bn_bwd_colsum(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma,
+                             const float* beta, const float* save_mean, const float* save_invstd, int relu, float* gx, int64_t ldgx,
+                             float* ggamma, float* gbeta, float* colsum, float drop_p, int64_t drop_seed, int64_t drop_layer,
+                             void* workspace, int64_t workspace_bytes, void* stream) {
+  PGNN_CHECK_ARG(M > 0 && C > 0 && M < (1ll << 31) && gy && x && gamma && beta && save_mean && save_invstd && gx && colsum && workspace);
+  PGNN_CHECK_ARG(ldgy >= C && ldx >= C && ldgx >= C);
+  PgnnDropout drop;
+  PGNN_CHECK_ARG(pgnn_make_dropout(drop_p, drop_seed, drop_layer, &drop));
+  if (workspace_bytes < pgnn_bn_workspace_bytes(M, C)) return PGNN_EWORKSPACE;
+  return pgnn_internal_bn_bwd_colsum(gy, ldgy, x, ldx, M, C, gamma, beta, save_mean, save_invstd, relu, gx, ldgx, ggamma, gbeta, colsum,
+                                     workspace, as_stream(stream), &drop);
 }
 
 }  // extern "C"

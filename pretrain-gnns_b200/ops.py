@@ -899,9 +899,29 @@ def chem_gin_relu_masks(plan: ChemEncoderPlan, gnn):
         masks.append(z1[l] > 0)
         if l != L - 1:
             bn = gnn.batch_norms[l]
-            xhat = (z2[l] - mean[l]) * invstd[l]
-            masks.append(torch.addcmul(bn.bias.detach(), xhat, bn.weight.detach()) > 0)   # the backward's own test: fma(xhat, gamma, beta) > 0
+            # the one BatchNorm pre-activation the forward's gather applied and the backward recomputes (common.cuh bn_preact):
+            # fmaf(z2, scale, shift) with scale = gamma * invstd, shift = fmaf(-mean, scale, beta).  Its sign is that of the exact
+            # z2 * scale + shift, which fp64 gives exactly (the product of two floats is exact there).
+            scale = bn.weight.detach() * invstd[l]
+            shift = fma32(-mean[l], scale, bn.bias.detach())
+            masks.append(z2[l].double() * scale.double() + shift.double() > 0)
     return masks
+
+
+def fma32(a, b, c):
+    """fp32 fmaf(a, b, c) of fp32 tensors, bit for bit (one rounding of the exact a * b + c).  The product is exact in fp64; the
+    fp64 sum s is rounded once more to fp32, which is the correctly rounded result unless s lands exactly halfway between two
+    floats, where the sign of the fp64 sum's own rounding error (TwoSum) decides."""
+    p, cd = a.double() * b.double(), c.double()
+    s = p + cd
+    bb = s - p
+    err = (p - (s - bb)) + (cd - bb)
+    f = s.float()
+    toward = torch.where(s > f.double(), torch.full_like(f, float("inf")), torch.full_like(f, float("-inf")))
+    nb = torch.nextafter(f, toward)
+    tie = (s != f.double()) & ((s - f.double()) * 2 == nb.double() - f.double())
+    past = tie & (err != 0) & ((err > 0) == (s > f.double()))
+    return torch.where(past, nb, f)
 
 
 # ------------------------------------------------------------------------------------------------

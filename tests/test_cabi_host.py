@@ -40,6 +40,39 @@ def test_argument_validation_without_gpu():
         cabi.check(-4, "x")
 
 
+def test_debug_bn_entries_validate_arguments_without_gpu():
+    """pgnn_debug_bn_apply_fold / pgnn_debug_bn_bwd_colsum reject bad sizes and row strides, missing pointers, a dropout p outside
+    [0, 1] and a short workspace before anything is enqueued (the fake addresses below are never dereferenced)."""
+    dll = cabi.lib.load()
+    P = 256  # a non-null address
+
+    def fold(M=8, C=4, x=P, sums=P, y=P, ldx=4, ldy=4, p=0.0):
+        return dll.pgnn_debug_bn_apply_fold(x, ldx, M, C, sums, P, P, None, None, None, 0.1, 1e-5, None, None, 1, y, ldy, p, 0, 0, None)
+
+    assert fold(M=0) == -1 and fold(C=0) == -1 and fold(M=1 << 31) == -1
+    assert fold(C=6145, ldx=6148, ldy=6148) == -1   # scale / shift of more columns than 48 KiB of shared memory holds
+    assert fold(x=None) == -1 and fold(sums=None) == -1 and fold(y=None) == -1
+    assert fold(ldx=3) == -1 and fold(ldy=3) == -1
+    assert fold(p=1.5) == -1 and fold(p=-0.1) == -1 and fold(p=float("nan")) == -1
+    wsb = dll.pgnn_bn_workspace_bytes(8, 4)
+    assert wsb > 0
+
+    def bwd(M=8, C=4, gy=P, colsum=P, ws=P, wsb=wsb, p=0.0, ldgy=4, ldx=4, ldgx=4):
+        return dll.pgnn_debug_bn_bwd_colsum(gy, ldgy, P, ldx, M, C, P, P, P, P, 1, P, ldgx, None, None, colsum, p, 0, 0, ws, wsb, None)
+
+    assert bwd(M=0) == -1 and bwd(C=0) == -1 and bwd(M=1 << 31) == -1
+    assert bwd(gy=None) == -1 and bwd(colsum=None) == -1 and bwd(ws=None) == -1
+    assert bwd(p=2.0) == -1
+    assert bwd(wsb=wsb - 1) == -3
+    assert bwd(ldgy=3) == -1 and bwd(ldx=3) == -1 and bwd(ldgx=3) == -1
+    # the whole-encoder gather's view of the workspace (GIN debug layout): additive to pgnn_chem_gin_debug_layout
+    off4 = (ctypes.c_int64 * 4)()
+    assert dll.pgnn_chem_gin_debug_layout(100, 200, 3, 300, off4) == 0
+    aggr = dll.pgnn_chem_gin_debug_aggr_offset(100, 200, 3, 300)
+    assert aggr > 0 and all(aggr + 3 * 100 * 300 * 4 <= o or o + 4 <= aggr for o in off4)
+    assert dll.pgnn_chem_gin_debug_aggr_offset(-1, 0, 3, 300) == -1 and dll.pgnn_chem_gin_debug_aggr_offset(10, 0, 0, 300) == -1
+
+
 @pytest.mark.parametrize("domain", ["chem", "bio"])
 @pytest.mark.parametrize("t", ["gin", "gcn", "graphsage", "gat"])
 def test_state_dict_contract(domain, t):

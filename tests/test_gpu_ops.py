@@ -182,10 +182,17 @@ def test_batch_norm_train(M, C, relu):
         assert int(edge.sum()) <= 8
         g_dev = torch.where(edge, x.grad, xd.grad.cpu())
         close(g_dev, x.grad, 1e-4 + 4e-4 * int(edge.any()), 1e-3)
+        # the parameter gradients sum R (times xhat) over the kept elements: count those edge elements as the GPU's forward took
+        # them (its y > 0, which its backward's mask equals), at the same tolerances
+        kept_dev, kept_cpu = yd.detach().cpu() > 0, pre.detach() > 0
+        dR = torch.where(edge, R * (kept_dev.float() - kept_cpu.float()), torch.zeros_like(R))
+        xhat = (x.detach() - x.detach().mean(0)) / torch.sqrt(x.detach().var(0, unbiased=False) + bn.eps)
+        gw_ref, gb_ref = bn.weight.grad + (dR * xhat).sum(0), bn.bias.grad + dR.sum(0)
     else:
         close(xd.grad, x.grad, 1e-4, 1e-3)
-    close(bd.weight.grad, bn.weight.grad, 1e-4 * M ** 0.5, 1e-4)
-    close(bd.bias.grad, bn.bias.grad, 1e-4 * M ** 0.5, 1e-4)
+        gw_ref, gb_ref = bn.weight.grad, bn.bias.grad
+    close(bd.weight.grad, gw_ref, 1e-4 * M ** 0.5, 1e-4)
+    close(bd.bias.grad, gb_ref, 1e-4 * M ** 0.5, 1e-4)
     close(bd.running_mean, bn.running_mean, 1e-5, 1e-5)
     close(bd.running_var, bn.running_var, 1e-5, 1e-5)
     assert int(bd.num_batches_tracked) == int(bn.num_batches_tracked) == 1
