@@ -265,6 +265,25 @@ PGNN_API int64_t pgnn_softmax_ce_rows_workspace_bytes(void);
 PGNN_API int pgnn_softmax_ce_rows_fwd(const float* logits, int64_t ld, int64_t M, int64_t V, const float* label_rows, int64_t ld_label,
                                       int64_t Q, double* loss_mean, float* dlogits, int64_t lddl, void* workspace,
                                       int64_t workspace_bytes, void* stream);
+/* Edge-prediction head (chem/pretrain_edgepred.py:31-41, bio/pretrain_edgepred.py): over x [N, ldx] fp32 (C columns),
+ *   pos_scores[p] = <x[pos_u[p * pos_stride]], x[pos_v[p * pos_stride]]>  (p < P; pos_u / pos_v: the two rows of
+ *                   edge_index[:, ::2], column stride pos_stride, no copy), neg_scores[q] likewise over the Q negative pairs,
+ *   *loss = mean_p BCE(pos_p, 1) + mean_q BCE(neg_q, 0)  (fp64; an empty side contributes NaN, as torch's empty mean does).
+ * Each dot product is an fp32 fmaf chain in a fixed order; dscore [P + Q] receives d loss / d score ((sigmoid - t) / P, then
+ * / Q); pairs [2, P + Q] int64 receives the pairs (positives first) for pgnn_graph_prep.  A pair with an endpoint outside
+ * [0, N) scores 0 and sets PGNN_DEVERR_GATHER.  C and ldx must be multiples of 4 and x 16-byte aligned.  Deterministic (per-CTA
+ * fp64 partials folded in order).  workspace: pgnn_edge_pair_bce_workspace_bytes() bytes, any content. */
+PGNN_API int64_t pgnn_edge_pair_bce_workspace_bytes(void);
+PGNN_API int pgnn_edge_pair_bce_fwd(const float* x, int64_t ldx, int64_t N, int64_t C, const int64_t* pos_u, const int64_t* pos_v,
+                                    int64_t pos_stride, int64_t P, const int64_t* neg_u, const int64_t* neg_v, int64_t neg_stride,
+                                    int64_t Q, double* loss, float* pos_scores, float* neg_scores, float* dscore, int64_t* pairs,
+                                    void* workspace, int64_t workspace_bytes, void* stream);
+/* Its backward: gx[i] = sum_{p: u_p = i} g_p x[v_p] + sum_{p: v_p = i} g_p x[u_p] with g_p = dscore[p] * (float)*gscale (gscale:
+ * device fp64 scalar, the gradient of the loss), each sum in pair order.  rowptr/nbr/eid _t and _s: pgnn_graph_prep of the
+ * `pairs` list over N nodes.  gx [N, ldgx] is OVERWRITTEN.  Deterministic, no atomics. */
+PGNN_API int pgnn_edge_pair_bce_bwd(const float* x, int64_t ldx, int64_t N, int64_t C, const float* dscore, const double* gscale,
+                                    const int32_t* rowptr_t, const int32_t* nbr_t, const int32_t* eid_t, const int32_t* rowptr_s,
+                                    const int32_t* nbr_s, const int32_t* eid_s, float* gx, int64_t ldgx, void* stream);
 /* out[r] = sum_d a[r,d] * b[(r + shift) mod B, d]   (cycle_index negatives, pretrain_contextpred.py:36-39,64-67) */
 PGNN_API int pgnn_shifted_rowdot_fwd(const float* a, int64_t lda, const float* b, int64_t ldb, int64_t B, int64_t C,
                                      int64_t shift, float* out, void* stream);
@@ -462,6 +481,21 @@ PGNN_API int pgnn_mask_edges_chem(const int64_t* edge_index, int64_t* edge_attr,
 PGNN_API int64_t pgnn_mask_edges_bio_count(const int64_t* edge_off_host, int64_t B, double mask_rate);
 PGNN_API int pgnn_mask_edges_bio(float* edge_attr, const int64_t* edge_off, int64_t B, double mask_rate, int64_t seed,
                                  int64_t* mask_off, int64_t* masked_edge_idx, float* mask_edge_label, void* stream);
+/* NegativeEdge (chem/util.py:22-52, bio/util.py:16-44) + BatchAE's node offset (chem/batch.py:69-121) on a batch collated by
+ * pgnn_collate_chem / pgnn_collate_bio (edge_index [2,E] int64 batch-global, node_off / edge_off [B+1]).  Per graph of n nodes
+ * and e columns, candidate j < 5e is (splitmix64(seed, 2 (5 edge_off[g] + j)) mod n, splitmix64(seed, 2 (5 edge_off[g] + j) + 1)
+ * mod n); it is accepted iff its endpoints differ, it is not a (directed) column of the graph and was not accepted before; the
+ * walk stops once e/2 are accepted when e is even (never when e is odd; n = 0 or e = 0 draws nothing).  negative_edge_index
+ * receives the accepted pairs + the graph's node offset as a contiguous [2, M] at its front (it must hold 2 * capacity int64),
+ * negative_edge_off [B+1] the exclusive scan of the per-graph counts (negative_edge_off[B] = M, the value the host reads back).
+ * capacity = pgnn_negative_edges_capacity(host copy of edge_off, B) = sum_g (e_g even ? e_g / 2 : 5 e_g).  A column endpoint
+ * outside its graph is ignored and sets PGNN_DEVERR_GATHER.  The workspace is linear in B, E and capacity.  Bit-exact against
+ * the host restatement of tests/edgepred_oracle.py. */
+PGNN_API int64_t pgnn_negative_edges_capacity(const int64_t* edge_off_host, int64_t B);
+PGNN_API int64_t pgnn_negative_edges_workspace_bytes(int64_t B, int64_t E, int64_t capacity);
+PGNN_API int pgnn_negative_edges(const int64_t* edge_index, int64_t E, const int64_t* node_off, const int64_t* edge_off, int64_t B,
+                                 int64_t seed, int64_t capacity, void* workspace, int64_t workspace_bytes, int64_t* negative_edge_index,
+                                 int64_t* negative_edge_off, void* stream);
 
 /* ExtractSubstructureContextPair + BatchSubstructContext.from_data_list on the device (chem/util.py:55-151 through
  * chem/loader.py:146-221, chem/batch.py:141-210; bio/util.py:123-205, bio/batch.py:196-265) for graphs held in HBM.

@@ -124,6 +124,46 @@ __host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t seed, uint64_t 
   return z ^ (z >> 31);
 }
 
+// Exclusive prefix of one flag across a CTA of kWarps full warps (every thread calls it); the CTA's total in `t`.  `sh` holds
+// kWarps ints of shared memory.  The transforms use it to give the selected items of a chunk their output ranks in order.
+template <int kWarps>
+__device__ __forceinline__ int block_scan_flag(bool a, int* sh, int& t) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned m = __ballot_sync(0xffffffffu, a);
+  __syncthreads();
+  if (lane == 0) sh[warp] = __popc(m);
+  __syncthreads();
+  int p = __popc(m & ((1u << lane) - 1u));
+  t = 0;
+#pragma unroll
+  for (int w = 0; w < kWarps; ++w) {
+    const int c = sh[w];
+    if (w < warp) p += c;
+    t += c;
+  }
+  return p;
+}
+
+// one warp: off[0..B] = exclusive scan of f(i)
+template <typename F>
+__device__ __forceinline__ void warp_scan_to(int64_t B, int64_t* __restrict__ off, F f) {
+  const int lane = threadIdx.x & 31;
+  int64_t carry = 0;
+  for (int64_t base = 0; base < B; base += 32) {
+    const int64_t i = base + lane;
+    const int64_t n = i < B ? f(i) : 0;
+    int64_t s = n;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int64_t t = __shfl_up_sync(0xffffffffu, s, d);
+      if (lane >= d) s += t;
+    }
+    if (i < B) off[i] = carry + s - n;
+    carry += __shfl_sync(0xffffffffu, s, 31);
+  }
+  if (lane == 0) off[B] = carry;
+}
+
 // Dropout of layer `layer`'s [rows, C] activation (include/pgnn_b200.h, pgnn_dropout_fwd): element (row i, column c) is kept
 // iff (splitmix64(seed, (layer << 40) | (i * C + c)) >> 32) >= thr, and then scaled by `scale`; a dropped element is multiplied
 // by 0 (so a dropped NaN / Inf gives NaN, as torch's x * mask * scale does).  The mask is regenerated wherever it is needed

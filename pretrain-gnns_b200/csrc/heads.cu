@@ -283,6 +283,138 @@ k_softmax_ce_rows(const float* __restrict__ logits, int64_t ld, int64_t M, int V
   }
 }
 
+// Edge prediction (chem/pretrain_edgepred.py:31-41, bio/pretrain_edgepred.py): pos_p = <x[u_p], x[v_p]> over the P positive
+// pairs, neg_q likewise over the Q negative ones, loss = mean_p BCE(pos_p, 1) + mean_q BCE(neg_q, 0).  A pair is held by 8 lanes
+// over float4 columns: lane l sums columns 4l, 4l+32, ... with fmaf in that order, and the 8 lane sums are folded by a fixed
+// xor-shuffle tree (deterministic).  The BCE terms and d loss / d score = (sigmoid(s) - t) / P (or / Q) are evaluated in fp64;
+// the loss is folded as k_softmax_ce_rows folds it (per-CTA fp64 partials summed in CTA order by the last CTA).  An empty side
+// gives torch's mean over nothing, NaN, and no gradient.  The same pass writes the P + Q pairs as one contiguous [2, P + Q]
+// list for pgnn_graph_prep, which buckets them for the backward.
+constexpr int kPairThreads = 256;
+constexpr int kPairsPerCta = kPairThreads / 8;
+constexpr int kPairMaxBlocks = kNumSMs * 8;
+
+struct PairBceWs {
+  double partial[2][kPairMaxBlocks];
+  unsigned int ticket;
+  unsigned int pad;
+};
+
+__global__ void __launch_bounds__(kPairThreads)
+k_edge_pair_bce_fwd(const float* __restrict__ x, int64_t ldx, int64_t N, int C4, const int64_t* __restrict__ pu, const int64_t* __restrict__ pv,
+                    int64_t ps, int64_t P, const int64_t* __restrict__ qu, const int64_t* __restrict__ qv, int64_t qs, int64_t Q,
+                    PairBceWs* __restrict__ ws, double* __restrict__ loss, float* __restrict__ pos, float* __restrict__ neg,
+                    float* __restrict__ dscore, int64_t* __restrict__ pairs, unsigned int* __restrict__ err) {
+  pdl_prologue();
+  __shared__ double s_part[2][kPairThreads / 32];
+  __shared__ bool s_last;
+  const int sub = threadIdx.x & 7;
+  const int64_t total = P + Q;
+  double acc[2] = {0.0, 0.0};
+  bool bad = false;
+  // `base` is uniform across the CTA: every lane runs every iteration and takes part in the group shuffles
+  for (int64_t base = (int64_t)blockIdx.x * kPairsPerCta; base < total; base += (int64_t)gridDim.x * kPairsPerCta) {
+    const int64_t p = base + (threadIdx.x >> 3);
+    const bool live = p < total, is_neg = p >= P;
+    int64_t u = 0, v = 0;
+    if (live) {
+      if (is_neg) u = qu[(p - P) * qs], v = qv[(p - P) * qs];
+      else u = pu[p * ps], v = pv[p * ps];
+    }
+    const bool ok = live && u >= 0 && u < N && v >= 0 && v < N;   // a pair outside [0, N) scores 0 and is flagged
+    float s = 0.f;
+    if (ok) {
+      const float* xu = x + u * ldx;
+      const float* xv = x + v * ldx;
+      for (int c = sub; c < C4; c += 8) {
+        const float4 a = ld4(xu + 4 * c), b = ld4(xv + 4 * c);
+        s = fmaf(a.x, b.x, s);
+        s = fmaf(a.y, b.y, s);
+        s = fmaf(a.z, b.z, s);
+        s = fmaf(a.w, b.w, s);
+      }
+    }
+#pragma unroll
+    for (int o = 4; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (live && sub == 0) {
+      bad |= !ok;
+      const double xs = (double)s, t = is_neg ? 0.0 : 1.0;
+      const double e = exp(-fabs(xs));
+      const double sig = xs >= 0.0 ? 1.0 / (1.0 + e) : e / (1.0 + e);
+      acc[is_neg] += fmax(xs, 0.0) - xs * t + log1p(e);
+      dscore[p] = (float)((sig - t) / (double)(is_neg ? Q : P));
+      if (is_neg) neg[p - P] = s;
+      else pos[p] = s;
+      pairs[p] = u;
+      pairs[total + p] = v;
+    }
+  }
+  if (bad && err) atomicOr(err, (unsigned)PGNN_DEVERR_GATHER);
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    double a = acc[k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if ((threadIdx.x & 31) == 0) s_part[k][threadIdx.x >> 5] = a;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double b0 = 0.0, b1 = 0.0;
+    for (int w = 0; w < kPairThreads / 32; ++w) b0 += s_part[0][w], b1 += s_part[1][w];
+    ws->partial[0][blockIdx.x] = b0;
+    ws->partial[1][blockIdx.x] = b1;
+    __threadfence();
+    s_last = atomicAdd(&ws->ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (s_last && threadIdx.x == 0) {
+    __threadfence();
+    double sp = 0.0, sq = 0.0;
+    for (unsigned b = 0; b < gridDim.x; ++b) {
+      sp += reinterpret_cast<volatile double*>(ws->partial[0])[b];
+      sq += reinterpret_cast<volatile double*>(ws->partial[1])[b];
+    }
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    *loss = (P > 0 ? sp / (double)P : nan) + (Q > 0 ? sq / (double)Q : nan);
+  }
+}
+
+// d x[i] = sum_{p: u_p = i} g_p x[v_p] + sum_{p: v_p = i} g_p x[u_p],  g_p = dscore[p] * (float)*gscale, each sum over the pairs
+// in pair order (the stable buckets of pgnn_graph_prep over the [2, P + Q] pair list: _t by u with payload v, _s by v with payload
+// u).  One thread per (row, float4 column), fmaf accumulation, no atomics: deterministic.  A pair with u = v sits in both buckets
+// of its row and contributes 2 g x[u].
+__global__ void __launch_bounds__(256)
+k_edge_pair_bce_bwd(const float* __restrict__ x, int64_t ldx, int64_t N, int C4, const float* __restrict__ dscore,
+                    const double* __restrict__ gscale, const int* __restrict__ rowptr_t, const int* __restrict__ nbr_t,
+                    const int* __restrict__ eid_t, const int* __restrict__ rowptr_s, const int* __restrict__ nbr_s,
+                    const int* __restrict__ eid_s, float* __restrict__ gx, int64_t ldgx) {
+  pdl_prologue();
+  const float gs = (float)*gscale;
+  const int64_t total = N * C4;
+  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t i = idx / C4;
+    const int c = (int)(idx - i * C4) * 4;
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int side = 0; side < 2; ++side) {
+      const int* rowptr = side ? rowptr_s : rowptr_t;
+      const int* nbr = side ? nbr_s : nbr_t;
+      const int* eid = side ? eid_s : eid_t;
+      const int lo = rowptr[i], hi = rowptr[i + 1];
+#pragma unroll 4
+      for (int k = lo; k < hi; ++k) {
+        const float g = __fmul_rn(dscore[eid[k]], gs);
+        const float4 v = ld4(x + (int64_t)nbr[k] * ldx + c);
+        acc.x = fmaf(g, v.x, acc.x);
+        acc.y = fmaf(g, v.y, acc.y);
+        acc.z = fmaf(g, v.z, acc.z);
+        acc.w = fmaf(g, v.w, acc.w);
+      }
+    }
+    st4(gx + i * ldgx + c, acc);
+  }
+}
+
 inline int grid_items(int64_t items, int threads) {
   int64_t b = ceil_div(items, threads);
   const int64_t cap = (int64_t)kNumSMs * 16;
@@ -387,6 +519,44 @@ int pgnn_softmax_ce_rows_fwd(const float* logits, int64_t ld, int64_t M, int64_t
     default: PGNN_CUDA(PGNN_CE_ROWS(32)); break;
   }
 #undef PGNN_CE_ROWS
+  PGNN_LAUNCH_CHECK();
+  return PGNN_OK;
+}
+
+int64_t pgnn_edge_pair_bce_workspace_bytes(void) { return (int64_t)sizeof(PairBceWs); }
+
+int pgnn_edge_pair_bce_fwd(const float* x, int64_t ldx, int64_t N, int64_t C, const int64_t* pos_u, const int64_t* pos_v, int64_t pos_stride,
+                           int64_t P, const int64_t* neg_u, const int64_t* neg_v, int64_t neg_stride, int64_t Q, double* loss,
+                           float* pos_scores, float* neg_scores, float* dscore, int64_t* pairs, void* workspace, int64_t workspace_bytes,
+                           void* stream) {
+  PGNN_CHECK_ARG(N >= 0 && C > 0 && ldx >= C && P >= 0 && Q >= 0 && loss && workspace);
+  PGNN_CHECK_ARG(P == 0 || (pos_u && pos_v && pos_scores));
+  PGNN_CHECK_ARG(Q == 0 || (neg_u && neg_v && neg_scores));
+  PGNN_CHECK_ARG(P + Q == 0 || (x && dscore && pairs));
+  if (workspace_bytes < (int64_t)sizeof(PairBceWs)) return PGNN_EWORKSPACE;
+  if (C % 4 || ldx % 4 || (x && !aligned16(x))) return PGNN_EUNSUPPORTED;
+  cudaStream_t st = as_stream(stream);
+  PairBceWs* ws = reinterpret_cast<PairBceWs*>(workspace);
+  PGNN_CUDA(cudaMemsetAsync(&ws->ticket, 0, sizeof(unsigned int), st));
+  int64_t blocks = ceil_div(P + Q, (int64_t)kPairsPerCta);
+  if (blocks > kPairMaxBlocks) blocks = kPairMaxBlocks;
+  if (blocks < 1) blocks = 1;   // one CTA writes the loss of an empty batch (NaN)
+  PGNN_CUDA(pgnn_launch(k_edge_pair_bce_fwd, dim3((unsigned)blocks), dim3(kPairThreads), 0, st, x, ldx, N, (int)(C / 4), pos_u, pos_v, pos_stride,
+                        P, neg_u, neg_v, neg_stride, Q, ws, loss, pos_scores, neg_scores, dscore, pairs, pgnn_error_flag_ptr()));
+  PGNN_LAUNCH_CHECK();
+  return PGNN_OK;
+}
+
+int pgnn_edge_pair_bce_bwd(const float* x, int64_t ldx, int64_t N, int64_t C, const float* dscore, const double* gscale,
+                           const int32_t* rowptr_t, const int32_t* nbr_t, const int32_t* eid_t, const int32_t* rowptr_s,
+                           const int32_t* nbr_s, const int32_t* eid_s, float* gx, int64_t ldgx, void* stream) {
+  PGNN_CHECK_ARG(N >= 0 && C > 0 && ldx >= C && ldgx >= C);
+  if (N == 0) return PGNN_OK;
+  PGNN_CHECK_ARG(x && gscale && rowptr_t && rowptr_s && gx);
+  if (C % 4 || ldx % 4 || ldgx % 4 || !aligned16(x) || !aligned16(gx)) return PGNN_EUNSUPPORTED;
+  const int C4 = (int)(C / 4);
+  PGNN_CUDA(pgnn_launch(k_edge_pair_bce_bwd, dim3(grid_items(N * C4, 256)), dim3(256), 0, as_stream(stream), x, ldx, N, C4, dscore, gscale,
+                        rowptr_t, nbr_t, eid_t, rowptr_s, nbr_s, eid_s, gx, ldgx));
   PGNN_LAUNCH_CHECK();
   return PGNN_OK;
 }

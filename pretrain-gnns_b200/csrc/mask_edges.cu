@@ -27,43 +27,7 @@ __device__ __forceinline__ int64_t edge_mask_count(int64_t pairs, double rate) {
   return k > pairs ? pairs : k;
 }
 
-// exclusive prefix of one flag across the CTA; total in `t`
-__device__ __forceinline__ int block_scan1(bool a, int* sh, int& t) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const unsigned m = __ballot_sync(0xffffffffu, a);
-  __syncthreads();
-  if (lane == 0) sh[warp] = __popc(m);
-  __syncthreads();
-  int p = __popc(m & ((1u << lane) - 1u));
-  t = 0;
-#pragma unroll
-  for (int w = 0; w < kWarps; ++w) {
-    const int c = sh[w];
-    if (w < warp) p += c;
-    t += c;
-  }
-  return p;
-}
-
-// one warp: off[0..B] = exclusive scan of f(i)
-template <typename F>
-__device__ __forceinline__ void warp_scan_to(int64_t B, int64_t* __restrict__ off, F f) {
-  const int lane = threadIdx.x & 31;
-  int64_t carry = 0;
-  for (int64_t base = 0; base < B; base += 32) {
-    const int64_t i = base + lane;
-    const int64_t n = i < B ? f(i) : 0;
-    int64_t s = n;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int64_t t = __shfl_up_sync(0xffffffffu, s, d);
-      if (lane >= d) s += t;
-    }
-    if (i < B) off[i] = carry + s - n;
-    carry += __shfl_sync(0xffffffffu, s, 31);
-  }
-  if (lane == 0) off[B] = carry;
-}
+__device__ __forceinline__ int block_scan1(bool a, int* sh, int& t) { return block_scan_flag<kWarps>(a, sh, t); }
 
 __global__ void __launch_bounds__(256)
 k_flag_nodes(const int64_t* __restrict__ idx, int64_t M, int64_t N, uint8_t* __restrict__ flags, unsigned int* __restrict__ err) {

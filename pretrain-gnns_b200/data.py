@@ -174,6 +174,30 @@ def mask_edges_bio(batch, edge_off_host, mask_rate=0.15, seed=0):
     return batch
 
 
+def negative_edges(batch, edge_off_host, seed=0):
+    """NegativeEdge (chem/util.py:22-52, bio/util.py:16-44) + BatchAE's offset (chem/batch.py:69-121, bio/batch.py:123-175) on a batch
+    collated by MoleculeStore.collate or BioGraphStore.collate, on the device: adds `negative_edge_index` [2, M] (batch-global ids)
+    and `negative_edge_off` [B+1].  Per graph of e columns, the first e/2 distinct valid pairs (all of them when e is odd) among
+    5e candidates drawn as pgnn_negative_edges defines.  `edge_off_host`: host copy of batch.edge_off (np.int64 [B+1]) to size
+    the output; M is data dependent, so one 8-byte read-back narrows the view.  `seed`: a fresh value per step."""
+    import ctypes
+    off = np.ascontiguousarray(edge_off_host, dtype=np.int64)
+    B = len(off) - 1
+    cap = int(check(lib.pgnn_negative_edges_capacity(off.ctypes.data_as(ctypes.c_void_p), B), "pgnn_negative_edges_capacity"))
+    ei = batch.edge_index.contiguous()
+    E, dev = int(ei.shape[1]), ei.device
+    wsb = int(check(lib.pgnn_negative_edges_workspace_bytes(B, E, cap), "pgnn_negative_edges_workspace_bytes"))
+    ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+    out = torch.empty((2 * max(cap, 1),), dtype=torch.int64, device=dev)
+    neg_off = torch.empty((B + 1,), dtype=torch.int64, device=dev)
+    check(lib.pgnn_negative_edges(ei.data_ptr(), E, batch.node_off.data_ptr(), batch.edge_off.data_ptr(), B, int(seed) & ((1 << 63) - 1), cap,
+                                  ws.data_ptr(), wsb, out.data_ptr(), neg_off.data_ptr(), torch.cuda.current_stream(dev).cuda_stream),
+          "pgnn_negative_edges")
+    M = int(neg_off[B])
+    batch.negative_edge_index, batch.negative_edge_off = out[:2 * M].view(2, M), neg_off
+    return batch
+
+
 def mask_edges_chem(batch, num_edge_type=5):
     """The mask_edge=True half of MaskAtom (chem/util.py:243-272) on a batch that mask_atoms has processed: adds
     `connected_edge_indices` [Mc], `mask_edge_label` [Mc,2] and overwrites the attribute rows of every bond touching a masked

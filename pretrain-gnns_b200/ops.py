@@ -1007,3 +1007,63 @@ def masked_edge_type_loss(node_rep, edge_index, masked_edge_idx, mask_edge_label
     A label past the V classes (the maximum in column 7 or 8) raises PGNN_DEVERR_LABEL.  -> (loss fp64, logits [M, V])."""
     me = edge_index.index_select(1, masked_edge_idx)
     return _MaskedCE.apply(node_rep, me[0], mask_edge_label, weight, bias, me[1])
+
+
+# ------------------------------------------------------------------------------------------------
+# edge-prediction head: pair dot products + BCE of both sides (chem/pretrain_edgepred.py:31-41) as one op
+# ------------------------------------------------------------------------------------------------
+def _pair_rows(index, name):
+    if index.dtype != torch.int64 or index.dim() != 2 or index.shape[0] != 2:
+        raise PgnnError("%s must be int64 [2, n]" % name)
+    m = int(index.shape[1])
+    if m == 0:
+        return None, None, 1, 0
+    return index[0].data_ptr(), index[1].data_ptr(), index.stride(1), m
+
+
+class _EdgePairBce(Function):
+    @staticmethod
+    def forward(ctx, node_rep, pos_index, neg_index):
+        _dev(node_rep, pos_index, neg_index)
+        x = _f32(node_rep)
+        if x.data_ptr() % 16 or x.stride(0) % 4:
+            x = x.contiguous()
+        N, C = x.shape
+        pu, pv, ps, P = _pair_rows(pos_index, "pos_index")
+        qu, qv, qs, Q = _pair_rows(neg_index, "neg_index")
+        dev = x.device
+        loss = torch.empty((), dtype=torch.float64, device=dev)
+        pos = torch.empty(P, dtype=torch.float32, device=dev)
+        neg = torch.empty(Q, dtype=torch.float32, device=dev)
+        dscore = torch.empty(P + Q, dtype=torch.float32, device=dev)
+        pairs = torch.empty(2, P + Q, dtype=torch.int64, device=dev)
+        wsb = int(lib.pgnn_edge_pair_bce_workspace_bytes())
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        check(lib.pgnn_edge_pair_bce_fwd(_p(x), x.stride(0), N, C, pu, pv, ps, P, qu, qv, qs, Q, _p(loss), _p(pos), _p(neg), _p(dscore),
+                                         _p(pairs), _p(ws), wsb, _st()), "edge_pair_bce_fwd")
+        ctx.graph = Graph(pairs, N) if ctx.needs_input_grad[0] else None   # both bucketings of the P + Q pairs, for the backward
+        ctx.save_for_backward(x, dscore)
+        ctx.mark_non_differentiable(pos, neg)
+        if _VALIDATE:
+            raise_on_device_errors()
+        return loss, pos, neg
+
+    @staticmethod
+    def backward(ctx, g, _g_pos, _g_neg):
+        x, dscore = ctx.saved_tensors
+        graph = ctx.graph
+        N, C = x.shape
+        g = g.to(torch.float64).contiguous()
+        gx = torch.empty(N, C, dtype=torch.float32, device=x.device)
+        check(lib.pgnn_edge_pair_bce_bwd(_p(x), x.stride(0), N, C, _p(dscore), _p(g), _p(graph.rowptr_t), _p(graph.nbr_t), _p(graph.eid_t),
+                                         _p(graph.rowptr_s), _p(graph.nbr_s), _p(graph.eid_s), _p(gx), C, _st()), "edge_pair_bce_bwd")
+        return gx, None, None
+
+
+def edge_pair_bce(node_rep, pos_index, neg_index):
+    """chem/pretrain_edgepred.py:35-39 (bio/pretrain_edgepred.py alike): pos = sum(node_rep[pos_index[0]] * node_rep[pos_index[1]], 1),
+    neg likewise over neg_index, loss = BCEWithLogits(pos, 1) + BCEWithLogits(neg, 0), each a mean over its own scores and
+    evaluated in fp64 (the script: fp32).  pos_index may be the strided view edge_index[:, ::2] (read in place).  An empty side
+    makes the loss NaN, as torch's mean over nothing does.  -> (loss fp64, pos [P] fp32, neg [Q] fp32; the scores are
+    non-differentiable, e.g. for the script's train_acc)."""
+    return _EdgePairBce.apply(node_rep, pos_index, neg_index)

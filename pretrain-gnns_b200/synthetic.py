@@ -282,3 +282,62 @@ def one_direction_only(batch: dict, seed: int, keys=("edge_index", "edge_attr"))
     out[keys[0]] = ei[:, keep].contiguous()
     out[keys[1]] = batch[keys[1]][keep].contiguous()
     return out
+
+
+def edge_offsets(batch: dict) -> np.ndarray:
+    """[B+1] np.int64 edge offsets of a zinc_batch / ppi_batch (edges are emitted graph by graph)."""
+    ptr, ei = batch["ptr"].numpy(), batch["edge_index"].numpy()
+    owner = np.searchsorted(ptr, ei[0], side="right") - 1
+    return np.searchsorted(owner, np.arange(len(ptr))).astype(np.int64)
+
+
+def negative_edge_index(edge_index, node_off, edge_off, seed: int) -> np.ndarray:
+    """NegativeEdge (chem/util.py:22-52) per graph + BatchAE's node offset, with the draw data.negative_edges makes on the device:
+    candidate j of graph g is (splitmix64(seed, 2 (5 e0 + j)) mod n, splitmix64(seed, 2 (5 e0 + j) + 1) mod n), e0 = edge_off[g],
+    j < 5e.  The reference's loop keeps, in candidate order, the first occurrence of every valid pair (endpoints differ, not a
+    directed column of the graph) and stops at e/2 of them when e is even; restated over the whole batch at once: np.unique's first
+    occurrences, then a per-graph cumulative count.  -> [2, M] int64 (batch-global ids)."""
+    ei = np.asarray(edge_index, dtype=np.int64)
+    node_off, edge_off = np.asarray(node_off, dtype=np.int64), np.asarray(edge_off, dtype=np.int64)
+    n, e = np.diff(node_off), np.diff(edge_off)
+    B = len(n)
+    K = np.where((n > 0) & (e > 0), 5 * e, 0)
+    if K.sum() == 0:
+        return np.zeros((2, 0), np.int64)
+    g = np.repeat(np.arange(B), K)
+    j = np.arange(int(K.sum()), dtype=np.int64) - np.repeat(np.cumsum(K) - K, K)
+    c = 2 * (5 * edge_off[g] + j)
+    ng = n[g].astype(np.uint64)
+    a = (splitmix64(seed, c) % ng).astype(np.int64)
+    b = (splitmix64(seed, c + 1) % ng).astype(np.int64)
+    W = int(n.max()) + 1
+    key = (g * W + a) * W + b
+    eg = np.repeat(np.arange(B), e)
+    u, v = ei[0] - node_off[eg], ei[1] - node_off[eg]
+    inside = (u >= 0) & (u < n[eg]) & (v >= 0) & (v < n[eg])
+    ekey = (eg[inside] * W + u[inside]) * W + v[inside]
+    cand = np.nonzero((a != b) & ~np.isin(key, ekey))[0]
+    _, first = np.unique(key[cand], return_index=True)
+    keep = np.sort(cand[first])
+    kg = g[keep]
+    rank = np.arange(len(keep)) - np.searchsorted(kg, kg)          # position among the graph's accepted pairs
+    keep = keep[(e[kg] % 2 == 1) | (rank < e[kg] // 2)]
+    return np.stack([node_off[g[keep]] + a[keep], node_off[g[keep]] + b[keep]])
+
+
+def edgepred_batch(num_graphs: int, seed: int, **zinc_kw) -> dict:
+    """chem/pretrain_edgepred.py's input: a zinc_batch after NegativeEdge and BatchAE (chem/batch.py:69-121), the negatives drawn
+    as data.negative_edges draws them under `seed`."""
+    b = zinc_batch(num_graphs, seed, **zinc_kw)
+    b["edge_off"] = _t(edge_offsets(b))
+    b["negative_edge_index"] = _t(negative_edge_index(b["edge_index"].numpy(), b["ptr"].numpy(), b["edge_off"].numpy(), seed))
+    return b
+
+
+def bio_edgepred_batch(num_graphs: int, seed: int, **ppi_kw) -> dict:
+    """bio/pretrain_edgepred.py's input: a ppi_batch after NegativeEdge and BatchAE (bio/batch.py:123-175), drawn as
+    edgepred_batch draws them."""
+    b = ppi_batch(num_graphs, seed, **ppi_kw)
+    b["edge_off"] = _t(edge_offsets(b))
+    b["negative_edge_index"] = _t(negative_edge_index(b["edge_index"].numpy(), b["ptr"].numpy(), b["edge_off"].numpy(), seed))
+    return b

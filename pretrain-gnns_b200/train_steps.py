@@ -15,6 +15,9 @@ restatement of the same bodies (oracle/steps_oracle.py) and with the reference's
                                                           masked edges' label rows (not in CONFIGS)
     BioContextPredStep bio/pretrain_contextpred.py:43-97  bio GNN(5,300) + GNN(3,300), cbow / mean pooling, BCE on fp64 scores
                                                           (not in CONFIGS)
+    EdgePredStep       chem/pretrain_edgepred.py:31-41    GNN(5,300,gnn_type), BCE of the dot products of the bonds and of the
+                                                          NegativeEdge pairs, on fp64 (not in CONFIGS)
+    BioEdgePredStep    bio/pretrain_edgepred.py           the same on bio GNN(5,300,gnn_type) (not in CONFIGS)
 """
 from __future__ import annotations
 
@@ -43,6 +46,8 @@ FINETUNE_KEYS = ("x", "edge_index", "edge_attr", "batch", "y")
 FINETUNE_SEED = 5  # seed = 5 * 1000 + 1000 * rank + batch index, in the scheme of make_batches
 BIO_MASKING_KEYS = ("x", "edge_index", "edge_attr", "masked_edge_idx", "mask_edge_label")
 BIO_MASKING_SEED, BIO_CONTEXT_SEED = 6, 7
+EDGEPRED_KEYS = ("x", "edge_index", "edge_attr", "negative_edge_index")
+EDGEPRED_SEED, BIO_EDGEPRED_SEED = 8, 9
 
 
 def make_batches(config, rank, count, batch_size=None, num_tasks=5000):
@@ -253,6 +258,47 @@ class BioContextPredStep(ContextPredStep):
         self.l1 = l1
         self.workload = ("bio pretrain_contextpred 5-layer GIN emb_dim=300 PPI-ego-shaped graphs batch_size=%d l1=%d, substruct + 3-layer "
                          "context encoder" % (batch_size, l1))
+
+
+class EdgePredStep(_Step):
+    """chem/pretrain_edgepred.py:31-41 with the script's defaults (num_layer 5, emb_dim 300, JK last, dropout 0, batch_size 256, any
+    gnn_type): node_emb = model(x, ei, ea); pos = sum(node_emb[ei[0, ::2]] * node_emb[ei[1, ::2]], 1), neg likewise over
+    negative_edge_index; loss = BCEWithLogits(pos, 1) + BCEWithLogits(neg, 0), evaluated in fp64 (the script: fp32)."""
+    encoder, source, seed_base, domain = chem.GNN, staticmethod(syn.edgepred_batch), EDGEPRED_SEED, "chem"
+
+    def __init__(self, device, gnn_type="gin", batch_size=256):
+        self.graphs_per_batch = batch_size
+        self.model = self.encoder(NUM_LAYER, EMB, JK="last", drop_ratio=0, gnn_type=gnn_type).to(device).train()
+        self.modules = [self.model]
+        self.workload = ("%s pretrain_edgepred 5-layer %s emb_dim=300 batch_size=%d"
+                         % (self.domain, gnn_type.upper() if gnn_type != "graphsage" else "GraphSAGE", batch_size))
+
+    KEYS = EDGEPRED_KEYS
+
+    def make_batches(self, rank, count):
+        return [_fields(self.source(self.graphs_per_batch, self.seed_base * 1000 + 1000 * rank + i), EDGEPRED_KEYS) for i in range(count)]
+
+    def flat_sources(self):
+        return [self.model]
+
+    def named_modules(self):
+        return {"model": self.model}
+
+    def scores(self, b):
+        """-> (loss, pos, neg): the loss and the two score vectors (the script's train_acc reads them)."""
+        rep = self.model(b["x"], b["edge_index"], b["edge_attr"])
+        return ops.edge_pair_bce(rep, b["edge_index"][:, ::2], b["negative_edge_index"])
+
+    def __call__(self, b):
+        self.zero_grad()
+        loss, _, _ = self.scores(b)
+        loss.backward()
+        return loss
+
+
+class BioEdgePredStep(EdgePredStep):
+    """bio/pretrain_edgepred.py: EdgePredStep's body on bio GNN(5, 300) over PPI ego graphs."""
+    encoder, source, seed_base, domain = bio.GNN, staticmethod(syn.bio_edgepred_batch), BIO_EDGEPRED_SEED, "bio"
 
 
 class FinetuneStep(_Step):
