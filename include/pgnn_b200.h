@@ -284,6 +284,38 @@ PGNN_API int pgnn_edge_pair_bce_fwd(const float* x, int64_t ldx, int64_t N, int6
 PGNN_API int pgnn_edge_pair_bce_bwd(const float* x, int64_t ldx, int64_t N, int64_t C, const float* dscore, const double* gscale,
                                     const int32_t* rowptr_t, const int32_t* nbr_t, const int32_t* eid_t, const int32_t* rowptr_s,
                                     const int32_t* nbr_s, const int32_t* eid_s, float* gx, int64_t ldgx, void* stream);
+/* Deep Graph Infomax head (chem/pretrain_deepgraphinfomax.py:61-73, bio/pretrain_deepgraphinfomax.py), csrc/infomax.cu.  Over
+ * node rows x [N, ldx] fp32 (C columns) of G graphs (batch: int64 [N] graph ids; seg_ptr [G+1] / seg_order [N] from
+ * pgnn_bucket(batch), as for pgnn_segment_mean_fwd; an id outside [0, G) has pgnn_bucket's precondition) and the
+ * Discriminator weight W [C, C] (contiguous):
+ *   S = sigmoid(segment mean of x)             [G, C]   pgnn_infomax_summary_fwd (an empty graph gives sigmoid(0) = 0.5)
+ *   H = S . W                                  [G, C]   the caller: pgnn_linear_bwd_x(gy = S, w = W)
+ *   pos[i] = <x_i, H[b_i]>, neg[i] = <x_i, H[(b_i + 1) mod G]>   (cycle_index(G, 1); G = 1 pairs a graph with itself)
+ *   *loss = mean_i BCE(pos_i, 1) + mean_i BCE(neg_i, 0)          pgnn_infomax_bce_fwd (fp64; N = 0 gives NaN)
+ * Each score is an fp32 fmaf chain over float4 columns in a fixed order; dscore [2N] receives d loss / d score ((sigmoid - 1) / N
+ * for pos, then sigmoid / N for neg).  H [G, C] contiguous.  C and ldx must be multiples of 4 and x, H 16-byte aligned (else
+ * PGNN_EUNSUPPORTED).  Deterministic (per-CTA fp64 partials folded in order).  workspace: pgnn_infomax_bce_workspace_bytes()
+ * bytes, any content. */
+PGNN_API int pgnn_infomax_summary_fwd(const float* x, int64_t ldx, const int32_t* seg_ptr, const int32_t* seg_order, int64_t G,
+                                      int64_t C, float* S, int64_t lds, void* stream);
+PGNN_API int64_t pgnn_infomax_bce_workspace_bytes(void);
+PGNN_API int pgnn_infomax_bce_fwd(const float* x, int64_t ldx, int64_t N, int64_t C, const int64_t* batch, const float* H, int64_t G,
+                                  double* loss, float* pos, float* neg, float* dscore, void* workspace, int64_t workspace_bytes,
+                                  void* stream);
+/* Its backward, with gscale the device fp64 upstream gradient of the loss (S, H as the forward left them, contiguous [G, C]):
+ *   dH[g] = gscale (sum_{i in g} dpos_i x_i + sum_{i in prev(g)} dneg_i x_i), prev(g) = (g - 1) mod G, rows in seg_order's
+ *           stable order, 8 partials per graph folded in order (no atomics);
+ *   gW    = S^T . dH   (pgnn_linear_bwd_w(gy = S, x = dH); at precision 1 its 3xTF32 GEMM with the split-K partials in the
+ *           workspace, folded in order);  dS = dH . W^T   (pgnn_linear_fwd(x = dH, w = W));
+ *   gx_i  = gscale (dpos_i H[b_i] + dneg_i H[(b_i + 1) mod G]) + dS[b_i] * S[b_i] * (1 - S[b_i]) / n_{b_i}, one pass.
+ * gx [N, ldgx] and gW [C, C] are OVERWRITTEN; either may be NULL (not computed).  precision as for pgnn_linear_*.  At 1 every
+ * output repeats bit for bit; at 0 gW inherits the FFMA weight-gradient GEMM's split-K atomics (G > 64: rounding-level jitter).
+ * workspace: pgnn_infomax_bce_bwd_workspace_bytes(G, C) bytes, 16-byte aligned, any content. */
+PGNN_API int64_t pgnn_infomax_bce_bwd_workspace_bytes(int64_t G, int64_t C);
+PGNN_API int pgnn_infomax_bce_bwd(const float* x, int64_t ldx, int64_t N, int64_t C, const int64_t* batch, const int32_t* seg_ptr,
+                                  const int32_t* seg_order, int64_t G, const float* S, const float* H, const float* W,
+                                  const float* dscore, const double* gscale, float* gx, int64_t ldgx, float* gW, int precision,
+                                  void* workspace, int64_t workspace_bytes, void* stream);
 /* out[r] = sum_d a[r,d] * b[(r + shift) mod B, d]   (cycle_index negatives, pretrain_contextpred.py:36-39,64-67) */
 PGNN_API int pgnn_shifted_rowdot_fwd(const float* a, int64_t lda, const float* b, int64_t ldb, int64_t B, int64_t C,
                                      int64_t shift, float* out, void* stream);

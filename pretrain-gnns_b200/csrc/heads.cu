@@ -9,48 +9,12 @@ namespace {
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
 
-// One CTA per (segment, chunk of 32 float4 columns): 8 row-lanes (warps) walk the segment's rows eight apart, four independent
-// row loads in flight each, and the eight partial sums are folded through shared memory in a fixed order (deterministic).  The
-// first version walked a segment's rows serially in one thread per float4 column: a chain of dependent-latency loads that took
-// 258 us for the 64 PPI ego graphs of ~500 nodes of the bio supervised step (a 38 MB read).
+// global_mean_pool: the segment-mean body of common.cuh (segment_mean_cta), shared with Deep Graph Infomax's summary.
 __global__ void __launch_bounds__(256)
 k_segment_mean_fwd(const float* __restrict__ x, int64_t ldx, const int* __restrict__ seg_ptr, const int* __restrict__ seg_order,
                    int64_t num_seg, int C4, float* __restrict__ out, int64_t ldo) {
   pdl_prologue();
-  __shared__ float4 red[8][32];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int64_t b = blockIdx.x;
-  const int c4 = blockIdx.y * 32 + lane;
-  const int lo = seg_ptr[b], hi = seg_ptr[b + 1];
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (c4 < C4) {
-    const float* xc = x + 4 * c4;
-    int k = lo + w;
-    for (; k + 24 < hi; k += 32) {
-      const float4 v0 = ld4(xc + (int64_t)seg_order[k] * ldx), v1 = ld4(xc + (int64_t)seg_order[k + 8] * ldx);
-      const float4 v2 = ld4(xc + (int64_t)seg_order[k + 16] * ldx), v3 = ld4(xc + (int64_t)seg_order[k + 24] * ldx);
-      acc.x += v0.x; acc.y += v0.y; acc.z += v0.z; acc.w += v0.w;
-      acc.x += v1.x; acc.y += v1.y; acc.z += v1.z; acc.w += v1.w;
-      acc.x += v2.x; acc.y += v2.y; acc.z += v2.z; acc.w += v2.w;
-      acc.x += v3.x; acc.y += v3.y; acc.z += v3.z; acc.w += v3.w;
-    }
-    for (; k < hi; k += 8) {
-      const float4 v = ld4(xc + (int64_t)seg_order[k] * ldx);
-      acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-    }
-  }
-  red[w][lane] = acc;
-  __syncthreads();
-  if (w == 0 && c4 < C4) {
-    float4 t = red[0][lane];
-#pragma unroll
-    for (int k = 1; k < 8; ++k) {
-      const float4 v = red[k][lane];
-      t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
-    }
-    const float cnt = (float)max(hi - lo, 1);  // count.clamp(min=1)
-    st4(out + b * ldo + 4 * c4, make_float4(t.x / cnt, t.y / cnt, t.z / cnt, t.w / cnt));
-  }
+  segment_mean_cta<false>(x, ldx, seg_ptr, seg_order, C4, out, ldo);
 }
 
 __global__ void __launch_bounds__(256)

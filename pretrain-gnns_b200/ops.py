@@ -1067,3 +1067,69 @@ def edge_pair_bce(node_rep, pos_index, neg_index):
     makes the loss NaN, as torch's mean over nothing does.  -> (loss fp64, pos [P] fp32, neg [Q] fp32; the scores are
     non-differentiable, e.g. for the script's train_acc)."""
     return _EdgePairBce.apply(node_rep, pos_index, neg_index)
+
+
+# ------------------------------------------------------------------------------------------------
+# Deep Graph Infomax head: summary, discriminator scores and both BCE terms (chem/pretrain_deepgraphinfomax.py:61-73) as one op
+# ------------------------------------------------------------------------------------------------
+class _InfomaxBce(Function):
+    @staticmethod
+    def forward(ctx, node_emb, weight, segs):
+        _dev(node_emb, weight)
+        x = _f32(node_emb)
+        if x.data_ptr() % 16 or x.stride(0) % 4:
+            x = x.contiguous()
+        w = _f32(weight).contiguous()
+        N, C = x.shape
+        G = segs.num_seg
+        if tuple(w.shape) != (C, C):
+            raise PgnnError("weight must be [%d, %d], got %s" % (C, C, tuple(w.shape)))
+        if segs.n != N:
+            raise PgnnError("batch has %d entries for %d node rows" % (segs.n, N))
+        dev = x.device
+        S = torch.empty(G, C, dtype=torch.float32, device=dev)
+        check(lib.pgnn_infomax_summary_fwd(_p(x), x.stride(0), _p(segs.ptr), _p(segs.order), G, C, _p(S), C, _st()), "infomax_summary_fwd")
+        H = torch.empty(G, C, dtype=torch.float32, device=dev)
+        check(lib.pgnn_linear_bwd_x(_p(S), C, _p(w), G, C, C, None, 0, _p(H), C, _precision, _st()), "linear_bwd_x")   # H = S . W
+        loss = torch.empty((), dtype=torch.float64, device=dev)
+        pos = torch.empty(N, dtype=torch.float32, device=dev)
+        neg = torch.empty(N, dtype=torch.float32, device=dev)
+        dscore = torch.empty(2 * N, dtype=torch.float32, device=dev)
+        wsb = int(lib.pgnn_infomax_bce_workspace_bytes())
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        check(lib.pgnn_infomax_bce_fwd(_p(x), x.stride(0), N, C, _p(segs.seg), _p(H), G, _p(loss), _p(pos), _p(neg), _p(dscore), _p(ws), wsb,
+                                       _st()), "infomax_bce_fwd")
+        ctx.segs = segs
+        ctx.save_for_backward(x, w, S, H, dscore)
+        ctx.mark_non_differentiable(pos, neg)
+        if _VALIDATE:
+            raise_on_device_errors()
+        return loss, pos, neg
+
+    @staticmethod
+    def backward(ctx, g, _g_pos, _g_neg):
+        x, w, S, H, dscore = ctx.saved_tensors
+        segs = ctx.segs
+        N, C = x.shape
+        G = segs.num_seg
+        g = g.to(torch.float64).contiguous()
+        gx = torch.empty(N, C, dtype=torch.float32, device=x.device) if ctx.needs_input_grad[0] else None
+        gw = torch.empty(C, C, dtype=torch.float32, device=x.device) if ctx.needs_input_grad[1] else None
+        wsb = int(lib.pgnn_infomax_bce_bwd_workspace_bytes(G, C))
+        ws = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+        check(lib.pgnn_infomax_bce_bwd(_p(x), x.stride(0), N, C, _p(segs.seg), _p(segs.ptr), _p(segs.order), G, _p(S), _p(H), _p(w), _p(dscore),
+                                       _p(g), _p(gx), C, _p(gw), _precision, _p(ws), wsb, _st()), "infomax_bce_bwd")
+        return gx, gw, None
+
+
+def infomax_bce(node_emb, batch, weight, num_graphs=None):
+    """chem/pretrain_deepgraphinfomax.py:61-73 (bio/pretrain_deepgraphinfomax.py alike) after the encoder:
+    summary = sigmoid(global_mean_pool(node_emb, batch)); pos_i = <node_emb_i, (summary @ weight)[batch_i]>, neg_i likewise against
+    the next graph's summary (cycle_index(G, 1)); loss = BCEWithLogits(pos, 1) + BCEWithLogits(neg, 0), each a mean over the N
+    nodes, evaluated in fp64 (the script: fp32).  `batch` is any vector global_mean_pool accepts (sorted or not); num_graphs=None
+    means batch.max() + 1, read back to the host as PyG 1.0.3 does.  Differentiable in node_emb and weight [D, D].  N = 0 makes
+    the loss NaN, as torch's mean over nothing does.  -> (loss fp64, pos [N] fp32, neg [N] fp32; the scores are
+    non-differentiable, e.g. for the script's train_acc)."""
+    if num_graphs is None:
+        num_graphs = int(batch.max().item()) + 1 if batch.numel() else 0  # same D2H sync PyG 1.0.3 performs
+    return _InfomaxBce.apply(node_emb, weight, Segments(batch, num_graphs))

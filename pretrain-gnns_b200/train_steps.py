@@ -18,9 +18,15 @@ restatement of the same bodies (oracle/steps_oracle.py) and with the reference's
     EdgePredStep       chem/pretrain_edgepred.py:31-41    GNN(5,300,gnn_type), BCE of the dot products of the bonds and of the
                                                           NegativeEdge pairs, on fp64 (not in CONFIGS)
     BioEdgePredStep    bio/pretrain_edgepred.py           the same on bio GNN(5,300,gnn_type) (not in CONFIGS)
+    InfomaxStep        chem/pretrain_deepgraphinfomax.py:59-74
+                                                          GNN(5,300,gnn_type) + Discriminator(300), BCE of each node's score
+                                                          against its graph's sigmoid mean-pool summary and the next graph's,
+                                                          on fp64 (not in CONFIGS)
+    BioInfomaxStep     bio/pretrain_deepgraphinfomax.py   the same on bio GNN(5,300,gnn_type) (not in CONFIGS)
 """
 from __future__ import annotations
 
+import math
 import types
 
 import torch
@@ -48,6 +54,8 @@ BIO_MASKING_KEYS = ("x", "edge_index", "edge_attr", "masked_edge_idx", "mask_edg
 BIO_MASKING_SEED, BIO_CONTEXT_SEED = 6, 7
 EDGEPRED_KEYS = ("x", "edge_index", "edge_attr", "negative_edge_index")
 EDGEPRED_SEED, BIO_EDGEPRED_SEED = 8, 9
+INFOMAX_KEYS = ("x", "edge_index", "edge_attr", "batch")
+INFOMAX_SEED, BIO_INFOMAX_SEED = 10, 11
 
 
 def make_batches(config, rank, count, batch_size=None, num_tasks=5000):
@@ -299,6 +307,73 @@ class EdgePredStep(_Step):
 class BioEdgePredStep(EdgePredStep):
     """bio/pretrain_edgepred.py: EdgePredStep's body on bio GNN(5, 300) over PPI ego graphs."""
     encoder, source, seed_base, domain = bio.GNN, staticmethod(syn.bio_edgepred_batch), BIO_EDGEPRED_SEED, "bio"
+
+
+class Discriminator(torch.nn.Module):
+    """The Discriminator of chem/pretrain_deepgraphinfomax.py:30-42 (bio alike): weight [D, D] drawn by
+    torch_geometric.nn.inits.uniform(D, weight), i.e. U(-1/sqrt(D), 1/sqrt(D)), so the same torch.manual_seed draws the same
+    values.  forward(x, summary) = sum(x * (summary @ weight), 1), as the script's; InfomaxStep calls ops.infomax_bce instead."""
+    def __init__(self, hidden_dim):
+        super().__init__()
+        self.weight = torch.nn.Parameter(torch.empty(hidden_dim, hidden_dim))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        bound = 1.0 / math.sqrt(self.weight.size(0))
+        self.weight.data.uniform_(-bound, bound)
+
+    def forward(self, x, summary):
+        return torch.sum(x * torch.matmul(summary, self.weight), dim=1)
+
+
+class InfomaxStep(_Step):
+    """chem/pretrain_deepgraphinfomax.py:59-74 with the script's defaults (num_layer 5, emb_dim 300, JK last, dropout 0, batch_size
+    256, any gnn_type): node_emb = gnn(x, ei, ea); summary = sigmoid(global_mean_pool(node_emb, batch)); pos / neg = the
+    Discriminator's scores against each node's own summary and against the next graph's (cycle_index(G, 1)); loss =
+    BCEWithLogits(pos, 1) + BCEWithLogits(neg, 0), evaluated in fp64 (the script: fp32).  The modules are named as Infomax names
+    them ('gnn', 'discriminator'), so load_state takes Infomax.state_dict()'s keys as they are."""
+    encoder, source, seed_base, domain = chem.GNN, staticmethod(syn.zinc_batch), INFOMAX_SEED, "chem"
+
+    def __init__(self, device, gnn_type="gin", batch_size=256):
+        self.graphs_per_batch = batch_size
+        self.gnn = self.encoder(NUM_LAYER, EMB, JK="last", drop_ratio=0, gnn_type=gnn_type).to(device).train()
+        self.discriminator = Discriminator(EMB).to(device)
+        self.modules = [self.gnn, self.discriminator]
+        self.workload = ("%s pretrain_deepgraphinfomax 5-layer %s emb_dim=300 batch_size=%d"
+                         % (self.domain, gnn_type.upper() if gnn_type != "graphsage" else "GraphSAGE", batch_size))
+
+    KEYS = INFOMAX_KEYS
+
+    def make_batches(self, rank, count):
+        """Host batches (INFOMAX_KEYS + 'num_graphs', an int: the graph count is known on the host, so the step reads nothing back)."""
+        out = []
+        for i in range(count):
+            b = self.source(self.graphs_per_batch, self.seed_base * 1000 + 1000 * rank + i)
+            out.append(_fields(b, INFOMAX_KEYS) | {"num_graphs": b["num_graphs"]})
+        return out
+
+    def flat_sources(self):
+        return [self.gnn]
+
+    def named_modules(self):
+        return {"gnn": self.gnn, "discriminator": self.discriminator}
+
+    def scores(self, b):
+        """-> (loss, pos, neg): the loss and the two score vectors (the script's train_acc reads them).  b["num_graphs"], when
+        present, is G; otherwise G = batch.max() + 1 is read back, as global_mean_pool does."""
+        node_emb = self.gnn(b["x"], b["edge_index"], b["edge_attr"])
+        return ops.infomax_bce(node_emb, b["batch"], self.discriminator.weight, b.get("num_graphs"))
+
+    def __call__(self, b):
+        self.zero_grad()
+        loss, _, _ = self.scores(b)
+        loss.backward()
+        return loss
+
+
+class BioInfomaxStep(InfomaxStep):
+    """bio/pretrain_deepgraphinfomax.py: InfomaxStep's body on bio GNN(5, 300) over PPI ego graphs."""
+    encoder, source, seed_base, domain = bio.GNN, staticmethod(syn.ppi_batch), BIO_INFOMAX_SEED, "bio"
 
 
 class FinetuneStep(_Step):
