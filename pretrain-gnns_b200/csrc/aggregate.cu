@@ -13,9 +13,6 @@
 
 namespace {
 
-__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
-__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
-
 __device__ __forceinline__ float4 affine_act(float4 v, const float* __restrict__ sc, const float* __restrict__ sh,
                                              int c, int relu) {
   if (sc) {
@@ -414,14 +411,6 @@ k_bio_embed_bwd(const float* __restrict__ x, const float* __restrict__ g, int64_
   atomicAdd(&gtab[c], a0);
   atomicAdd(&gtab[C + c], a1);
 }
-
-inline int grid_items(int64_t items, int threads) {
-  int64_t b = ceil_div(items, threads);
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  if (b > cap) b = cap;
-  return (int)(b < 1 ? 1 : b);
-}
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 }  // namespace
 

@@ -215,6 +215,18 @@ struct TcEpilogue {
 // H100 SXM: 132 SMs.  Grids for grid-stride kernels are sized as a multiple of this.
 constexpr int kNumSMs = 132;
 
+// blocks of `threads` for a grid-stride kernel over `items` work items: one item per thread, capped at 16 blocks per SM
+static inline int grid_items(int64_t items, int threads) {
+  int64_t b = ceil_div(items, threads);
+  const int64_t cap = (int64_t)kNumSMs * 16;
+  if (b > cap) b = cap;
+  return (int)(b < 1 ? 1 : b);
+}
+
+static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
+
 // Programmatic dependent launch (PDL).  Every kernel of this library starts with pdl_prologue(): wait until the
 // previous kernel in the stream has completed and flushed (griddepcontrol.wait), then allow the NEXT kernel's CTAs to
 // become resident (griddepcontrol.launch_dependents) so that its launch latency and prologue overlap this kernel's

@@ -505,8 +505,6 @@ k_colsum_tc(const float* __restrict__ gy, int64_t ld, int M, int N, int rows_per
   }
 }
 
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 template <bool A_KC, bool B_KC, int BN>
 int launch(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N, int K, int splits,
            int k_per_split, const TcEpilogue& ep, cudaStream_t st) {

@@ -18,13 +18,6 @@ k_dropout(const float* __restrict__ x, int64_t ldx, int64_t M, int64_t C, PgnnDr
   }
 }
 
-inline int grid_items(int64_t items, int threads) {
-  int64_t b = ceil_div(items, threads);
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  if (b > cap) b = cap;
-  return (int)(b < 1 ? 1 : b);
-}
-
 // forward and backward are the same map: y = x * factor(l, i, c)
 int dropout_apply(const float* x, int64_t ldx, int64_t M, int64_t C, float p, int64_t seed, int64_t layer, float* y, int64_t ldy,
                   void* stream) {

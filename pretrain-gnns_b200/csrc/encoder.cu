@@ -51,17 +51,14 @@ int pgnn_internal_transpose_batch(int count, const float* const* in, float* cons
                                   cudaStream_t st);
 int pgnn_internal_bn_apply_fold(const float* x, int64_t ldx, int64_t M, int64_t C, const PgnnBnFold& fold, int relu, float* y,
                                 int64_t ldy, cudaStream_t st, const PgnnDropout* drop);
-int pgnn_internal_bn_bwd_colsum(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma,
-                                const float* beta, const float* save_mean, const float* save_invstd, int relu, float* gx,
-                                int64_t ldgx, float* ggamma, float* gbeta, float* colsum, void* workspace, cudaStream_t st,
-                                const PgnnDropout* drop);
 int pgnn_internal_bn_fwd_train(const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma, const float* beta,
                                float* running_mean, float* running_var, int64_t* num_batches_tracked, float momentum, float eps,
                                int relu, float* y, int64_t ldy, float* save_mean, float* save_invstd, float* scale, float* shift,
                                void* workspace, int64_t workspace_bytes, void* stream, const PgnnDropout* drop);
 int pgnn_internal_bn_bwd(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma,
                          const float* beta, const float* save_mean, const float* save_invstd, int relu, float* gx, int64_t ldgx,
-                         float* ggamma, float* gbeta, void* workspace, int64_t workspace_bytes, void* stream, const PgnnDropout* drop);
+                         float* ggamma, float* gbeta, float* colsum, void* workspace, int64_t workspace_bytes, cudaStream_t st,
+                         const PgnnDropout* drop);
 
 namespace {
 
@@ -460,9 +457,9 @@ int gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg
     // of mlp.2.bias
     if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad2 has finished reading this copy
     const PgnnDropout drop = drops.at(l);
-    TRY(pgnn_internal_bn_bwd_colsum(gy, ldgy, z2, D, N, D, (const float*)p[L_GAMMA], (const float*)p[L_BETA], w.mean + l * D,
-                                    w.invstd + l * D, !last, gz2, D, grads + o[L_GAMMA], grads + o[L_BETA], grads + o[L_B2],
-                                    w.scratch, st, &drop));
+    TRY(pgnn_internal_bn_bwd(gy, ldgy, z2, D, N, D, (const float*)p[L_GAMMA], (const float*)p[L_BETA], w.mean + l * D,
+                             w.invstd + l * D, !last, gz2, D, grads + o[L_GAMMA], grads + o[L_BETA], grads + o[L_B2],
+                             w.scratch, w.scratch_bytes, st, &drop));
     // MLP backward.  On the tensor path the dgrad epilogues carry the column reductions that would otherwise be
     // passes of their own: colsum(gz1) = gradient of mlp.0.bias, and S^T gaggr = gradient of the two bond tables.
     bool fused = false;
@@ -612,7 +609,8 @@ int conv_backward(int conv_type, const void* const* params, const float* g_node_
     const float* beta = (const float*)p[gat ? A_BETA : G_BETA];
     const PgnnDropout drop = drops.at(l);
     TRY(pgnn_internal_bn_bwd(gy, ldgy, z, D, N, D, gamma, beta, w.mean + l * D, w.invstd + l * D, !last, w.gz, D,
-                             grads + o[gat ? A_GAMMA : G_GAMMA], grads + o[gat ? A_BETA : G_BETA], w.scratch, w.scratch_bytes, stream, &drop));
+                             grads + o[gat ? A_GAMMA : G_GAMMA], grads + o[gat ? A_BETA : G_BETA], nullptr, w.scratch, w.scratch_bytes, st,
+                             &drop));
     if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad has finished reading this copy of gxl
     if (gat) {
       // gT [9, HD] lands on the two adjacent bond-table gradients

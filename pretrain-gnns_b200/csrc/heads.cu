@@ -6,9 +6,6 @@
 
 namespace {
 
-__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
-__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
-
 // global_mean_pool: the segment-mean body of common.cuh (segment_mean_cta), shared with Deep Graph Infomax's summary.
 __global__ void __launch_bounds__(256)
 k_segment_mean_fwd(const float* __restrict__ x, int64_t ldx, const int* __restrict__ seg_ptr, const int* __restrict__ seg_order,
@@ -378,14 +375,6 @@ k_edge_pair_bce_bwd(const float* __restrict__ x, int64_t ldx, int64_t N, int C4,
     st4(gx + i * ldgx + c, acc);
   }
 }
-
-inline int grid_items(int64_t items, int threads) {
-  int64_t b = ceil_div(items, threads);
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  if (b > cap) b = cap;
-  return (int)(b < 1 ? 1 : b);
-}
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 }  // namespace
 

@@ -15,9 +15,6 @@ int64_t pgnn_tc_wgrad_workspace_floats(int64_t M, int64_t N, int64_t K);
 
 namespace {
 
-__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
-__device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
-
 __global__ void __launch_bounds__(256)
 k_infomax_summary_fwd(const float* __restrict__ x, int64_t ldx, const int* __restrict__ seg_ptr, const int* __restrict__ seg_order,
                       int C4, float* __restrict__ S, int64_t lds) {
@@ -199,13 +196,6 @@ k_infomax_node_bwd(int64_t N, int C4, const int64_t* __restrict__ batch, const i
   }
 }
 
-inline int grid_items(int64_t items, int threads) {
-  int64_t b = ceil_div(items, threads);
-  const int64_t cap = (int64_t)kNumSMs * 16;
-  if (b > cap) b = cap;
-  return (int)(b < 1 ? 1 : b);
-}
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 inline int64_t gc_bytes(int64_t G, int64_t C) { return align_up(G * C * (int64_t)sizeof(float), 256); }
 
 }  // namespace
