@@ -348,6 +348,8 @@ PGNN_API int pgnn_bce_logits_fwd(const float* logits, int64_t ld, int64_t M, int
  *   training mode exactly as torch.nn.BatchNorm1d does; bn_num_batches_tracked may be NULL).
  * workspace: device scratch of pgnn_chem_gin_workspace_bytes; forward leaves the bucketed graph and the saved
  *   activations in it, backward consumes them, so the SAME workspace must be passed to both.
+ * precision: backward must get the forward's (what the forward saves depends on it: the tensor-path backward reads the one-hot
+ *   atom-code rows that only a precision = 1 training forward writes).
  * grads: ONE flat fp32 buffer; tensor i of the params order lives at [offsets[i], offsets[i+1]) with offsets from
  *   pgnn_chem_gin_grad_offsets (host array of num_params + 1 entries).  OVERWRITTEN.
  * ------------------------------------------------------------------------------------------- */
@@ -435,8 +437,8 @@ PGNN_API int pgnn_chem_conv_backward(int conv_type, const void* const* params, c
  * last layer, its ReLU) is multiplied by the pgnn_dropout_fwd mask of (drop_p, drop_seed, layer = l).  It never makes a pass of
  * its own: the kernel that writes or loads layer l's output applies it (GIN: the next layer's gather and the BatchNorm apply of
  * node_rep; the conv types: the BatchNorm apply that writes the layer's output), and the backward applies it to the incoming
- * gradient inside the BatchNorm backward.  Eval mode (training = 0) applies none; backward must get the forward's drop_p and
- * drop_seed.  drop_p == 0 is exactly pgnn_chem_gin_* / pgnn_chem_conv_*, which pass it.  Workspace, parameter and gradient
+ * gradient inside the BatchNorm backward.  Eval mode (training = 0) applies none; backward must get the forward's drop_p,
+ * drop_seed and precision.  drop_p == 0 is exactly pgnn_chem_gin_* / pgnn_chem_conv_*, which pass it.  Workspace, parameter and gradient
  * layouts are those of the type's own entry points; backward's edge_attr is only read for GAT.  gnn_type outside {0, 1, 2, 3},
  * drop_p outside [0, 1] or NaN: PGNN_EINVAL. */
 PGNN_API int pgnn_chem_encoder_forward(int gnn_type, const void* const* params, void* const* bn_running_mean,

@@ -27,6 +27,7 @@
 #include <cstdlib>
 #include <map>
 #include <mutex>
+#include <vector>
 
 int pgnn_internal_edge_table_bwd2(const float* S, int Q, const float* g, int64_t ldg, int64_t g_off, int64_t n, int C, float* gT,
                                   int64_t ldt, float* gT2, int q_split, cudaStream_t st);
@@ -413,12 +414,13 @@ int gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg
                  int64_t D, const Drops& drops, int precision, float* grads, void* workspace, int64_t workspace_bytes, void* stream) {
   PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && grads && workspace);
   if (workspace_bytes < pgnn_chem_gin_workspace_bytes(N, E, L, D)) return PGNN_EWORKSPACE;
-  int64_t off[2 + L_COUNT * 64 + 1];
-  PGNN_CHECK_ARG(L <= 64);
-  grad_layout(kGin, L, D, off);
+  const int64_t count = grad_layout(kGin, L, D, nullptr);
+  std::vector<int64_t> offsets(count + 1);
+  const int64_t* off = offsets.data();
+  grad_layout(kGin, L, D, offsets.data());
   cudaStream_t st = as_stream(stream);
   if (N == 0) {
-    PGNN_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * off[2 + L_COUNT * L], st));
+    PGNN_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * off[count], st));
     return PGNN_OK;
   }
   PGNN_CHECK_ARG(g_node_rep && x);
@@ -578,16 +580,18 @@ int conv_forward(int conv_type, const void* const* params, void* const* bn_runni
 int conv_backward(int conv_type, const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x,
                   const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, const Drops& drops, int precision, float* grads,
                   void* workspace, int64_t workspace_bytes, void* stream) {
-  PGNN_CHECK_ARG(valid_conv(conv_type) && N >= 0 && E >= 0 && L >= 1 && L <= 64 && D > 0 && D % 4 == 0 && params && grads && workspace);
+  PGNN_CHECK_ARG(valid_conv(conv_type) && N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && grads && workspace);
   if (workspace_bytes < pgnn_chem_conv_workspace_bytes(conv_type, N, E, L, D)) return PGNN_EWORKSPACE;
-  int64_t off[2 + A_COUNT * 64 + 1];
-  grad_layout(conv_type, L, D, off);
+  const int64_t count = grad_layout(conv_type, L, D, nullptr);
+  std::vector<int64_t> offsets(count + 1);
+  const int64_t* off = offsets.data();
+  grad_layout(conv_type, L, D, offsets.data());
   cudaStream_t st = as_stream(stream);
   const bool gat = conv_type == PGNN_CONV_GAT;
   const int64_t HD = gat ? kHeads * D : D;
   const int PL = layer_params(conv_type);
   if (N == 0) {
-    PGNN_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * off[2 + PL * L], st));
+    PGNN_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * off[count], st));
     return PGNN_OK;
   }
   PGNN_CHECK_ARG(g_node_rep && x && (E == 0 || edge_attr));

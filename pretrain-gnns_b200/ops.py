@@ -760,14 +760,16 @@ class ChemEncoderPlan:
             self._ws_alloc = ((need + need // 16) + (16 << 20) - 1) // (16 << 20) * (16 << 20)
         return self._ws_alloc
 
-    def forward(self, ptrs, rm, rv, nbt, x, ei, ea, N, E, training, momentum, eps, drop_p, drop_seed, out, ws, wsb):
+    def forward(self, ptrs, rm, rv, nbt, x, ei, ea, N, E, training, momentum, eps, drop_p, drop_seed, precision, out, ws, wsb):
         check(lib.pgnn_chem_encoder_forward(self.conv, ptrs, rm, rv, nbt, _p(x), _p(ei), _p(ea), N, E, self.L, self.D, int(training),
-                                            float(momentum), float(eps), float(drop_p), int(drop_seed), _precision, _p(out), self.D,
+                                            float(momentum), float(eps), float(drop_p), int(drop_seed), precision, _p(out), self.D,
                                             _p(ws), wsb, _st()), "chem_encoder_forward")
 
-    def backward(self, ptrs, g, x, ea, N, E, drop_p, drop_seed, flat, ws, wsb):
+    def backward(self, ptrs, g, x, ea, N, E, drop_p, drop_seed, precision, flat, ws, wsb):
+        """`precision` must be the one the forward ran with: the backward reads what that forward saved in `ws` (the tensor path
+        also the one-hot atom-code rows, which only a tf32x3 training forward writes)."""
         check(lib.pgnn_chem_encoder_backward(self.conv, ptrs, _p(g), g.stride(0), _p(x), _p(ea), N, E, self.L, self.D, float(drop_p),
-                                             int(drop_seed), _precision, _p(flat), _p(ws), wsb, _st()), "chem_encoder_backward")
+                                             int(drop_seed), precision, _p(flat), _p(ws), wsb, _st()), "chem_encoder_backward")
 
 
 def _deliver_flat_grads(plan, ctx, run):
@@ -849,9 +851,11 @@ class _ChemEncoder(Function):
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
         out = torch.empty(N, D, dtype=torch.float32, device=dev)
         mom = bns[0].momentum if bns[0].momentum is not None else 0.1
-        plan.forward(ptrs, rm, rv, nbt, x, ei, ea, N, E, training, mom, bns[0].eps, drop_p, drop_seed, out, ws, wsb)
+        precision = _precision
+        plan.forward(ptrs, rm, rv, nbt, x, ei, ea, N, E, training, mom, bns[0].eps, drop_p, drop_seed, precision, out, ws, wsb)
         ctx.plan, ctx.ws, ctx.wsb, ctx.ptrs, ctx.x, ctx.ea, ctx.dims, ctx.training = plan, ws, wsb, ptrs, x, ea, (N, E), training
         ctx.drop = (drop_p, drop_seed)  # the backward regenerates the masks from these
+        ctx.precision = precision       # and reads the workspace this precision's forward wrote, whatever set_precision says by then
         ctx.keep = params  # the pointer table refers to these storages
         if training and plan.keep_workspace:
             plan.last_ws = (ws, (N, E, plan.L, D))
@@ -871,7 +875,8 @@ class _ChemEncoder(Function):
         plan = ctx.plan
         N, E = ctx.dims
         g = _f32(g)
-        out = _deliver_flat_grads(plan, ctx, lambda flat: plan.backward(ctx.ptrs, g, ctx.x, ctx.ea, N, E, *ctx.drop, flat, ctx.ws, ctx.wsb))
+        out = _deliver_flat_grads(plan, ctx, lambda flat: plan.backward(ctx.ptrs, g, ctx.x, ctx.ea, N, E, *ctx.drop, ctx.precision, flat,
+                                                                          ctx.ws, ctx.wsb))
         _release_ctx(ctx)
         return out
 

@@ -54,7 +54,8 @@ def layer_masks(seed, num_layer, rows, C, p, dtype=torch.float64):
 
 
 def _drop(h, masks, l, p):
-    return h if masks is None else h * masks[l].to(h.dtype) * (1.0 / (1.0 - p))
+    """The library's factor: the fp32 scale(p), which is 0 at p = 1 (every element dropped) rather than 0 * inf."""
+    return h if masks is None else h * masks[l].to(h.dtype) * scale(p)
 
 
 def chem_gnn(P, x, edge_index, edge_attr, num_layer, gnn_type="gin", training=False, new_stats=None, pre="", masks=None, p=0.0):
@@ -68,7 +69,7 @@ def chem_gnn(P, x, edge_index, edge_attr, num_layer, gnn_type="gin", training=Fa
         h = conv(P, lp, h, ei, O.chem_edge_rows(P, lp, edge_attr, n))
         h = O.batch_norm(P, f"{pre}batch_norms.{l}.", h, training, new_stats)
         if l != num_layer - 1:
-            h = torch.relu(h)
+            h = O._relu(h)  # traced (O.RELU_TRACE) like the oracle's own ReLUs
         h = _drop(h, masks, l, p)
     return h
 
