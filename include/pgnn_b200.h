@@ -453,6 +453,48 @@ PGNN_API int pgnn_chem_encoder_backward(int gnn_type, const void* const* params,
                                         int64_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Whole-encoder entry points of the bio GNN (bio/model.py:11-290, JK="last", any drop_ratio): the same two-call contract as
+ * pgnn_chem_encoder_* for gnn_type 0 = GIN and PGNN_CONV_GCN / _SAGE / _GAT.
+ *
+ * Per layer: layer 0 embeds the dummy label x [N] (float-coded 0 / 1) with input_node_embeddings [2, D].  Each conv's edge encoder
+ * Linear(9, C) (C = 2D for GAT, else D) acts through the summary S [N,10] of pgnn_bio_edge_summary (self-loop bit at column 7); the
+ * library builds its [10, C] table [W^T ; b] itself.
+ *   GIN:  message [x_j || e_ij] (2D wide), MLP Linear(2D,2D) -> BatchNorm1d(2D) -> ReLU -> Linear(2D,D);
+ *   GCN / GraphSAGE (+ L2 normalisation) / GAT (2 heads, slope 0.2): Linear, then the conv as in the chem block.
+ * There is no outer BatchNorm.  Every layer but the last is followed by ReLU; in training with drop_p > 0, layer l's output is then
+ * multiplied by the pgnn_dropout_fwd mask of (drop_p, drop_seed, layer = l).  Eval mode (training = 0) applies none.
+ *
+ * params: HOST array of num_params = 1 + P*L DEVICE pointers
+ *   [gnns.0.input_node_embeddings.weight [2,D], then per layer gnns.l.
+ *    gin  (P = 8): mlp.0.weight [2D,2D], mlp.0.bias [2D], mlp.1.weight [2D], mlp.1.bias [2D], mlp.3.weight [D,2D], mlp.3.bias [D],
+ *                  edge_encoder.weight [D,9], edge_encoder.bias [D]
+ *    gcn / graphsage (P = 4): linear.weight [D,D], linear.bias [D], edge_encoder.weight [D,9], edge_encoder.bias [D]
+ *    gat  (P = 6): weight_linear.weight [2D,D], weight_linear.bias [2D], att [1,2,2D], bias [D], edge_encoder.weight [2D,9],
+ *                  edge_encoder.bias [2D]]
+ * bn_running_mean / bn_running_var / bn_num_batches_tracked: HOST arrays of L device pointers, the inner BatchNorm1d(2D) of each
+ *   GIN layer (gnns.l.mlp.1), updated in training mode as torch does; num_batches_tracked may be NULL.  Ignored (may be NULL) for
+ *   the other types.
+ * workspace: pgnn_bio_encoder_workspace_bytes; the SAME workspace goes to forward and backward.  The backward must get the
+ *   forward's drop_p, drop_seed and precision.
+ * grads: ONE flat fp32 buffer, tensor i of the params order (in the parameter's own shape) at [offsets[i], offsets[i+1]) of
+ *   pgnn_bio_encoder_grad_offsets (host array of num_params + 1 entries).  OVERWRITTEN.  backward's edge_attr is only read for GAT.
+ * D % 4 == 0.  gnn_type outside {0, 1, 2, 3}, L < 1, drop_p outside [0, 1] or NaN: PGNN_EINVAL.  A short workspace: PGNN_EWORKSPACE.
+ * ------------------------------------------------------------------------------------------- */
+PGNN_API int64_t pgnn_bio_encoder_num_params(int gnn_type, int64_t L);
+PGNN_API int pgnn_bio_encoder_grad_offsets(int gnn_type, int64_t L, int64_t D, int64_t* offsets);
+PGNN_API int64_t pgnn_bio_encoder_workspace_bytes(int gnn_type, int64_t N, int64_t E, int64_t L, int64_t D);
+PGNN_API int pgnn_bio_encoder_forward(int gnn_type, const void* const* params, void* const* bn_running_mean,
+                                      void* const* bn_running_var, void* const* bn_num_batches_tracked, const float* x /*[N]*/,
+                                      const int64_t* edge_index, const float* edge_attr /*[E,9]*/, int64_t N, int64_t E, int64_t L,
+                                      int64_t D, int training, float momentum, float eps, float drop_p, int64_t drop_seed,
+                                      int precision, float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes,
+                                      void* stream);
+PGNN_API int pgnn_bio_encoder_backward(int gnn_type, const void* const* params, const float* g_node_rep, int64_t ldg,
+                                       const float* x, const float* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D,
+                                       float drop_p, int64_t drop_seed, int precision, float* grads, void* workspace,
+                                       int64_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Either side of the path inside a training step (SURVEY.md section 8(f): f1 collation, f2 optimizer).
  * ------------------------------------------------------------------------------------------- */
 /* Device-side batch collation for chem graphs: what BatchMasking.from_data_list / BatchSubstructContext do on the host

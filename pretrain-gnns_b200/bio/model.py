@@ -131,10 +131,34 @@ class GNN(nn.Module):
             raise ValueError("unknown gnn_type %r" % (gnn_type,))
         self.num_layer, self.drop_ratio, self.JK = num_layer, drop_ratio, JK
         self.gnns = nn.ModuleList([_CONVS[gnn_type](emb_dim, l == 0) for l in range(num_layer)])
+        self._gnn_type = gnn_type
+        self._plan = None          # lazily built bookkeeping of the whole-encoder path (ops.BioEncoderPlan)
+        self.fused = True          # set False to force the layer-by-layer composition (used by the tests)
+
+    _DEFAULT_AGGR = {"gin": "add", "gcn": "add", "gat": "add", "graphsage": "mean"}
+
+    def _fused_plan(self):
+        """The whole-encoder kernels (pgnn_bio_encoder_*) cover every gnn_type with JK='last', the conv's default aggregation
+        (and GAT's 2 heads / slope 0.2), with or without dropout."""
+        if not (self.fused and self.JK == "last"):
+            return None
+        if any(conv.aggr != self._DEFAULT_AGGR[self._gnn_type] for conv in self.gnns):
+            return None
+        if self._gnn_type == "gin" and any(conv.mlp[1].training != self.training for conv in self.gnns):
+            return None
+        if self._gnn_type == "gat" and any(conv.heads != 2 or conv.negative_slope != 0.2 for conv in self.gnns):
+            return None
+        if self._plan is None:
+            self._plan = ops.BioEncoderPlan(self, self._gnn_type)
+        return self._plan
 
     def forward(self, x, edge_index, edge_attr):
-        graph = ops.graph_for(edge_index, x.size(0))
         drop = self.training and self.drop_ratio > 0
+        plan = self._fused_plan()
+        if plan is not None:
+            seed = ops.draw_seed() if drop else 0  # the same draw as below: both paths drop the same units
+            return ops.bio_encoder(plan, x, edge_index, edge_attr, self.training, self.drop_ratio if drop else 0.0, seed)
+        graph = ops.graph_for(edge_index, x.size(0))
         seed = ops.draw_seed() if drop else 0  # one per forward; layer l's mask is ops.dropout's of (seed, l)
         h = x
         hs = []

@@ -22,6 +22,9 @@
 // Parameters arrive as a host array of device pointers in a fixed order, gradients leave in ONE flat fp32 buffer with the
 // library-defined layout of pgnn_chem_gin_grad_offsets / pgnn_chem_conv_grad_offsets (grad_layout below), which is also the
 // buffer the data-parallel all-reduce runs on.
+//
+// The bio GNN (bio/model.py, pgnn_bio_encoder_*) has its own layer bodies at the end of the file on the same scaffolding:
+// workspace carving (Carve / Front), Drops, the side-stream weight gradients (SideCtx) and a flat gradient layout.
 #include "common.cuh"
 
 #include <cstdlib>
@@ -151,7 +154,8 @@ struct Front {
   float* onehot;         // [N, kOneHotLd]: atom-code one-hot rows (embedding gradient as a GEMM)
 };
 
-void carve_front(Carve& c, Front& f, int type, int64_t N, int64_t E, int64_t D) {
+// Q: the summary's columns (9 chem, 10 bio); onehot_ld: the one-hot rows' width (0: none, bio)
+void carve_front(Carve& c, Front& f, int type, int64_t N, int64_t E, int64_t D, int64_t Q = 9, int64_t onehot_ld = kOneHotLd) {
   const int64_t e1 = E > 0 ? E : 1;
   f.rowptr_t = c.take<int32_t>(N + 1);
   f.rowptr_s = c.take<int32_t>(N + 1);
@@ -159,10 +163,10 @@ void carve_front(Carve& c, Front& f, int type, int64_t N, int64_t E, int64_t D) 
   f.eid_t = c.take<int32_t>(e1);
   f.nbr_s = c.take<int32_t>(e1);
   f.eid_s = c.take<int32_t>(e1);
-  f.S = c.take<float>(N * 9);
+  f.S = c.take<float>(N * Q);
   f.dinv = type == kGin ? nullptr : c.take<float>(N);
   f.h0 = c.take<float>(N * D);
-  f.onehot = c.take<float>(N * kOneHotLd);
+  f.onehot = onehot_ld ? c.take<float>(N * onehot_ld) : nullptr;
 }
 
 // split-K partial tiles for the largest weight-gradient GEMM of a type: its layer wgrads ([N_out, D] with N_out = the given
@@ -653,6 +657,492 @@ int conv_backward(int conv_type, const void* const* params, const float* g_node_
   return embed_backward(sc, w, w.gh, x, N, D, precision, grads, off, w.wpart, w.wpart_floats, st);
 }
 
+// ==============================================================================================================================
+// bio (bio/model.py:11-290 with JK="last", any drop_ratio)
+// ==============================================================================================================================
+// Layer 0 embeds the dummy node label (input_node_embeddings [2, D]).  Each conv's edge encoder Linear(9, C) acts through the
+// per-node summary S [N, 10] (pgnn_bio_edge_summary) and the table T [10, C] = [W^T ; b]: the forward packs every layer's table in
+// one launch, and the backward scatters every layer's table gradient back as the encoder's weight [C, 9] and bias [C] in one.
+//   GIN        aggr = [sum_j x_j || S.T] (2D wide), then Linear(2D,2D) -> BatchNorm1d(2D) -> ReLU -> Linear(2D,D)
+//   GCN / GraphSAGE / GAT: as for chem, with the bio table (GAT reads the 9 float attributes per edge).
+// There is no outer BatchNorm: every layer but the last is followed by ReLU, then by layer l's dropout mask.  GIN applies both on
+// load in the next layer's gather (and, under dropout, its last layer takes one dropout sweep that writes node_rep); the conv
+// types take one ReLU + dropout sweep per layer that writes the layer's output (bio_act).  The backward runs the matching sweep
+// on the incoming gradient of every layer.
+
+constexpr int kBioQ = 10;       // S columns: the 9 edge attributes + the weight sum that multiplies the encoder bias
+constexpr int kBioEmbRows = 2;  // input_node_embeddings
+constexpr int kMaxPack = 64;    // layers per table-pack launch (their pointers travel as kernel arguments)
+
+// order of the bio parameter pointer table and of its flat gradient layout (one enum, so the types' indices mix in expressions)
+enum BioParam {
+  PB_EMB = 0, PB_LAYER0 = 1,
+  BG_W1 = 0, BG_B1, BG_GAMMA, BG_BETA, BG_W2, BG_B2, BG_ENC_W, BG_ENC_B, BG_COUNT,  // gin: mlp.0, mlp.1, mlp.3, edge_encoder
+  BC_W = 0, BC_B, BC_ENC_W, BC_ENC_B, BC_COUNT,                                     // gcn / graphsage
+  BA_W = 0, BA_B, BA_ATT, BA_BIAS, BA_ENC_W, BA_ENC_B, BA_COUNT                     // gat
+};
+
+inline int bio_layer_params(int type) { return type == kGin ? BG_COUNT : type == PGNN_CONV_GAT ? BA_COUNT : BC_COUNT; }
+inline int bio_enc_w(int type) { return type == kGin ? BG_ENC_W : type == PGNN_CONV_GAT ? BA_ENC_W : BC_ENC_W; }
+inline int64_t bio_width(int type, int64_t D) { return type == PGNN_CONV_GAT ? kHeads * D : D; }  // C: the edge encoder's width
+bool valid_type(int t) { return t == kGin || valid_conv(t); }
+
+int64_t bio_grad_layout(int type, int64_t L, int64_t D, int64_t* offsets) {
+  if (!offsets) return 1 + (int64_t)bio_layer_params(type) * L;
+  const int64_t C = bio_width(type, D);
+  int64_t o = 0, i = 0;
+  auto next = [&](int64_t size) { offsets[i++] = o; o += size; };
+  next(kBioEmbRows * D);  // gnns.0.input_node_embeddings.weight
+  for (int64_t l = 0; l < L; ++l) {
+    if (type == kGin) {
+      next(4 * D * D);  // mlp.0.weight [2D, 2D]
+      next(2 * D);      // mlp.0.bias
+      next(2 * D);      // mlp.1.weight (BatchNorm1d(2D))
+      next(2 * D);      // mlp.1.bias
+      next(2 * D * D);  // mlp.3.weight [D, 2D]
+      next(D);          // mlp.3.bias
+    } else {
+      next(C * D);  // linear.weight / weight_linear.weight [C, D]
+      next(C);      // its bias
+      if (type == PGNN_CONV_GAT) {
+        next(kHeads * 2 * D);  // att [1, H, 2D]
+        next(D);               // bias [D]
+      }
+    }
+    next(9 * C);  // edge_encoder.weight [C, 9]
+    next(C);      // edge_encoder.bias (adjacent: the table gradient scatter writes both)
+  }
+  offsets[i] = o;
+  return i;
+}
+
+struct PackArgs {
+  const float* w[kMaxPack];
+  const float* b[kMaxPack];
+};
+
+// T[l][q][c] = W_l[c][q] for q < 9, T[l][9][c] = b_l[c]: `count` layers' edge encoders as the [10, C] tables the kernels index
+__global__ void __launch_bounds__(256) k_bio_pack_tables(PackArgs a, int count, int C, float* __restrict__ T) {
+  pdl_prologue();
+  const int64_t per = (int64_t)kBioQ * C, total = per * count;
+  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int l = (int)(idx / per);
+    const int r = (int)(idx - l * per);
+    const int q = r / C, c = r - q * C;
+    T[idx] = q < 9 ? a.w[l][c * 9 + q] : a.b[l][c];
+  }
+}
+
+// the transpose: gT [L][10][C] -> every layer's edge_encoder.weight [C, 9] and .bias [C] gradients, layer l's at out + l * stride
+__global__ void __launch_bounds__(256) k_bio_unpack_table_grads(const float* __restrict__ gT, int64_t L, int C, float* __restrict__ out,
+                                                                int64_t stride) {
+  pdl_prologue();
+  const int64_t per = (int64_t)kBioQ * C, total = per * L;
+  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t l = idx / per;
+    const int r = (int)(idx - l * per);
+    const int q = r / C, c = r - q * C;
+    out[l * stride + (q < 9 ? (int64_t)c * 9 + q : (int64_t)9 * C + c)] = gT[idx];
+  }
+}
+
+// The inter-layer activation of bio/model.py:278-286 as one sweep.  Forward (BWD = false): y = relu(x) (relu != 0; NaN kept)
+// times layer d.layer's dropout factor.  Backward (BWD = true): gx = (relu ? (z > 0 ? gy : 0) : gy) times the same factor, z the
+// forward's pre-activation.  DROP = false has no hash.  One warp per row, VEC (4: float4, 1: scalar, for strides that are not a
+// multiple of 4) columns per lane.
+__device__ __forceinline__ float bio_act1(float v, float z, bool bwd, int relu) {
+  return relu ? (bwd ? (z > 0.f ? v : 0.f) : relu_keep_nan(v)) : v;
+}
+
+template <bool BWD, bool DROP, int VEC>
+__global__ void __launch_bounds__(256) k_bio_act(const float* __restrict__ x, int64_t ldx, const float* __restrict__ z, int64_t ldz,
+                                                 int64_t M, int64_t C, int relu, PgnnDropout d, float* __restrict__ y, int64_t ldy) {
+  pdl_prologue();
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t r = blockIdx.x * (int64_t)(blockDim.x >> 5) + (threadIdx.x >> 5); r < M; r += warps) {
+    for (int64_t c = (int64_t)lane * VEC; c < C; c += 32 * VEC) {
+      if (VEC == 4) {
+        float4 v = ld4(x + r * ldx + c);
+        const float4 zz = BWD && relu ? ld4(z + r * ldz + c) : v;
+        v.x = bio_act1(v.x, zz.x, BWD, relu);
+        v.y = bio_act1(v.y, zz.y, BWD, relu);
+        v.z = bio_act1(v.z, zz.z, BWD, relu);
+        v.w = bio_act1(v.w, zz.w, BWD, relu);
+        if (DROP) v = dropout4(v, d, r, C, c);
+        st4(y + r * ldy + c, v);
+      } else {
+        float v = bio_act1(x[r * ldx + c], BWD && relu ? z[r * ldz + c] : 0.f, BWD, relu);
+        if (DROP) v *= dropout_factor(d, r, C, c);
+        y[r * ldy + c] = v;
+      }
+    }
+  }
+}
+
+int bio_act(bool bwd, const float* x, int64_t ldx, const float* z, int64_t ldz, int64_t M, int64_t C, int relu, const PgnnDropout& d,
+            float* y, int64_t ldy, cudaStream_t st) {
+  const bool drop = d.p > 0.f;
+  const bool v4 = C % 4 == 0 && ldx % 4 == 0 && ldy % 4 == 0 && aligned16(x) && aligned16(y) &&
+                  (!(bwd && relu) || (ldz % 4 == 0 && aligned16(z)));
+  auto k = v4 ? (bwd ? (drop ? k_bio_act<true, true, 4> : k_bio_act<true, false, 4>) : (drop ? k_bio_act<false, true, 4> : k_bio_act<false, false, 4>))
+              : (bwd ? (drop ? k_bio_act<true, true, 1> : k_bio_act<true, false, 1>) : (drop ? k_bio_act<false, true, 1> : k_bio_act<false, false, 1>));
+  PGNN_CUDA(pgnn_launch(k, dim3(grid_items(M * 32, 256)), dim3(256), 0, st, x, ldx, z, ldz, M, C, relu, d, y, ldy));
+  PGNN_LAUNCH_CHECK();
+  return PGNN_OK;
+}
+
+// the backward's gradient at layer l's pre-activation: the incoming rows themselves when the layer has neither ReLU nor dropout
+// and the consumers can read them in place (16-byte rows), else the bio_act sweep into `buf`
+int bio_act_bwd(const float*& gz, int64_t& ldgz, const float* gy, int64_t ldgy, const float* z, int64_t M, int64_t D, bool last,
+                const PgnnDropout& d, float* buf, cudaStream_t st) {
+  if (last && d.p == 0.f && ldgy % 4 == 0 && aligned16(gy)) {
+    gz = gy;
+    ldgz = ldgy;
+    return PGNN_OK;
+  }
+  gz = buf;
+  ldgz = D;
+  return bio_act(true, gy, ldgy, z, D, M, D, !last, d, buf, D, st);
+}
+
+int bio_pack_tables(int type, const void* const* params, int64_t L, int64_t C, float* T, cudaStream_t st) {
+  const int PL = bio_layer_params(type), ew = bio_enc_w(type);
+  for (int64_t l0 = 0; l0 < L; l0 += kMaxPack) {
+    const int count = (int)(L - l0 < kMaxPack ? L - l0 : kMaxPack);
+    PackArgs a{};
+    for (int i = 0; i < count; ++i) {
+      const void* const* p = params + PB_LAYER0 + (l0 + i) * PL;
+      a.w[i] = (const float*)p[ew];
+      a.b[i] = (const float*)p[ew + 1];
+      PGNN_CHECK_ARG(a.w[i] && a.b[i]);
+    }
+    PGNN_CUDA(pgnn_launch(k_bio_pack_tables, dim3(grid_items(kBioQ * C * count, 256)), dim3(256), 0, st, a, count, (int)C,
+                          T + l0 * kBioQ * C));
+    PGNN_LAUNCH_CHECK();
+  }
+  return PGNN_OK;
+}
+
+struct BioGinWs : Front {
+  float* T;                      // [L][10][D] packed edge-encoder tables
+  double* bn_acc;                // [L][2][2D] fp64 sums of the inner BatchNorm (tensor path)
+  float *mean, *invstd;          // [L, 2D]
+  float *aggr, *z1, *y1, *z2;    // per layer: gather [N, 2D], Linear 1 [N, 2D], BatchNorm + ReLU [N, 2D], Linear 2 [N, D]
+  float *gz2, *gy1, *gz1, *ga;   // backward temporaries; gz2 and gz1 two copies by layer parity (side-stream wgrad operands)
+  float *gh, *gT;                // [N, D], [L][10][D]
+  float* wpart;
+  int64_t wpart_floats;
+  void* scratch;
+  int64_t scratch_bytes, total;
+};
+
+BioGinWs carve_bio_gin(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
+  Carve c(base, false);
+  BioGinWs w;
+  const int64_t D2 = 2 * D;
+  carve_front(c, w, kGin, N, E, D, kBioQ, 0);
+  w.T = c.take<float>(L * kBioQ * D);
+  w.bn_acc = c.take<double>(L * 2 * D2);
+  w.mean = c.take<float>(L * D2);
+  w.invstd = c.take<float>(L * D2);
+  w.aggr = c.take<float>(L * N * D2);
+  w.z1 = c.take<float>(L * N * D2);
+  w.y1 = c.take<float>(L * N * D2);
+  w.z2 = c.take<float>(L * N * D);
+  w.gz2 = c.take<float>(2 * N * D);
+  w.gy1 = c.take<float>(N * D2);
+  w.gz1 = c.take<float>(2 * N * D2);
+  w.ga = c.take<float>(N * D2);
+  w.gh = c.take<float>(N * D);
+  w.gT = c.take<float>(L * kBioQ * D);
+  const int64_t a = pgnn_tc_wgrad_workspace_floats(N, D2, D2), b = pgnn_tc_wgrad_workspace_floats(N, D, D2);
+  w.wpart_floats = a > b ? a : b;
+  w.wpart = c.take<float>(w.wpart_floats);
+  int64_t sb = pgnn_graph_prep_workspace_bytes(N, E);
+  const int64_t bb = pgnn_bn_workspace_bytes(N > 0 ? N : 1, D2);
+  if (bb > sb) sb = bb;
+  w.scratch_bytes = sb;
+  w.scratch = c.take<char>(sb);
+  w.total = c.off;
+  return w;
+}
+
+struct BioConvWs : Front {
+  float *T, *xl, *z, *hout;    // [L][10][C]; per layer: Linear output [N, C], conv output [N, D], after ReLU + dropout [N, D]
+  float *nrm, *alpha, *pq;     // per layer: SAGE row norms [N]; GAT attention [(E+N), H] and logit halves [N, H, 2]
+  float *gz, *ga, *gxl, *gh;   // backward temporaries [N, D], [N, D], two copies of [N, C] by layer parity, [N, D]
+  float* gT;                   // [L][10][C]
+  float* wpart;
+  int64_t wpart_floats;
+  void* scratch;
+  int64_t scratch_bytes, total;
+};
+
+BioConvWs carve_bio_conv(void* base, int type, int64_t N, int64_t E, int64_t L, int64_t D) {
+  Carve c(base, true);
+  BioConvWs w;
+  const int64_t C = bio_width(type, D);
+  carve_front(c, w, type, N, E, D, kBioQ, 0);
+  w.T = c.take<float>(L * kBioQ * C);
+  w.xl = c.take<float>(L * N * C);
+  w.z = c.take<float>(L * N * D);
+  w.hout = c.take<float>(L * N * D);
+  w.nrm = c.take<float>(type == PGNN_CONV_SAGE ? L * N : 0);
+  w.alpha = c.take<float>(type == PGNN_CONV_GAT ? L * (E + N) * kHeads : 0);
+  w.pq = c.take<float>(type == PGNN_CONV_GAT ? L * N * kHeads * 2 : 0);
+  w.gz = c.take<float>(N * D);
+  w.ga = c.take<float>(N * D);
+  w.gxl = c.take<float>(2 * N * C);
+  w.gh = c.take<float>(N * D);
+  w.gT = c.take<float>(L * kBioQ * C);
+  w.wpart_floats = pgnn_tc_wgrad_workspace_floats(N, C, D);
+  w.wpart = c.take<float>(w.wpart_floats);
+  int64_t sb = pgnn_graph_prep_workspace_bytes(N, E);
+  if (type == PGNN_CONV_GAT) {
+    const int64_t gb = pgnn_gat_bwd_workspace_bytes(N, E, kHeads, D);
+    if (gb > sb) sb = gb;
+  }
+  w.scratch_bytes = sb;
+  w.scratch = c.take<char>(sb);
+  w.total = c.off;
+  return w;
+}
+
+int64_t bio_workspace_bytes(int type, int64_t N, int64_t E, int64_t L, int64_t D) {
+  return type == kGin ? carve_bio_gin(nullptr, N, E, L, D).total : carve_bio_conv(nullptr, type, N, E, L, D).total;
+}
+
+// Graph preparation, the summary S (not for GAT, whose kernels read the attributes per edge), the label embedding and every
+// layer's packed edge-encoder table.
+int bio_prologue(int type, const Front& f, float* T, const void* const* params, const float* x, const int64_t* edge_index,
+                 const float* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, void* scratch, int64_t scratch_bytes, cudaStream_t st) {
+  TRY(pgnn_graph_prep(edge_index, E, N, f.rowptr_t, f.nbr_t, f.eid_t, f.rowptr_s, f.nbr_s, f.eid_s, scratch, scratch_bytes, st));
+  if (type == PGNN_CONV_GCN) TRY(pgnn_gcn_dinv(f.rowptr_t, N, f.dinv, st));
+  if (type != PGNN_CONV_GAT) TRY(pgnn_bio_edge_summary(edge_attr, f.rowptr_t, f.nbr_t, f.eid_t, N, agg_mode(type), f.dinv, f.S, st));
+  TRY(pgnn_bio_embed_fwd(x, (const float*)params[PB_EMB], N, D, f.h0, D, st));
+  return bio_pack_tables(type, params, L, bio_width(type, D), T, st);
+}
+
+// One weight-gradient GEMM of the bio backward: gw [Nout, K] = gy^T x and gb = the column sums of gy (gb may be null), on the side
+// stream when there is one, ordered by the context's event pair k of this layer parity (SideCtx).  A shape the tensor path does
+// not cover runs on the caller's stream once everything on the side stream has finished.
+int side_wgrad(const SideCtx* sc, cudaStream_t st, int k, int par, int precision, const float* gy, int64_t ldgy, const float* x,
+               int64_t ldx, int64_t M, int64_t Nout, int64_t K, float* gw, float* gb, float* wpart, int64_t wpart_floats) {
+  cudaStream_t wst = sc ? sc->side : st;
+  if (sc) {
+    PGNN_CUDA(cudaEventRecord(sc->ready[k][par], st));
+    PGNN_CUDA(cudaStreamWaitEvent(wst, sc->ready[k][par], 0));
+  }
+  int rc = PGNN_EUNSUPPORTED;
+  if (precision == 1) rc = pgnn_tc_linear_bwd_w_ws(gy, ldgy, x, ldx, M, Nout, K, gw, gb, wpart, wpart_floats, wst);
+  if (rc == PGNN_EUNSUPPORTED) {
+    if (sc) TRY(join_side(sc, st));
+    return pgnn_linear_bwd_w(gy, ldgy, x, ldx, M, Nout, K, gw, gb, precision, st);
+  }
+  if (rc == PGNN_OK && sc) PGNN_CUDA(cudaEventRecord(sc->done[k][par], wst));
+  return rc;
+}
+
+// Backward tail of every bio type: the side stream joins, then the label-embedding gradient and the edge-encoder gradients of
+// every layer from the table gradients gT [L][10][C].
+int bio_backward_tail(int type, const SideCtx* sc, const float* gT, const float* gh, const float* x, int64_t N, int64_t L, int64_t D,
+                      float* grads, const int64_t* off, cudaStream_t st) {
+  if (sc) TRY(join_side(sc, st));
+  TRY(pgnn_bio_embed_bwd(x, gh, D, N, D, grads + off[PB_EMB], st));
+  const int64_t C = bio_width(type, D);
+  const int64_t stride = off[PB_LAYER0 + bio_layer_params(type)] - off[PB_LAYER0];
+  PGNN_CUDA(pgnn_launch(k_bio_unpack_table_grads, dim3(grid_items(L * kBioQ * C, 256)), dim3(256), 0, st, gT, L, (int)C,
+                        grads + off[PB_LAYER0 + bio_enc_w(type)], stride));
+  PGNN_LAUNCH_CHECK();
+  return PGNN_OK;
+}
+
+int bio_gin_forward(const void* const* params, void* const* bn_running_mean, void* const* bn_running_var, void* const* bn_num_batches_tracked,
+                    int64_t N, int64_t L, int64_t D, int training, float momentum, float eps, const Drops& drops, int precision,
+                    float* node_rep, int64_t ld_out, const BioGinWs& w, cudaStream_t st) {
+  const int64_t D2 = 2 * D;
+  for (int64_t l = 0; l < L; ++l) {
+    const void* const* p = params + PB_LAYER0 + l * BG_COUNT;
+    float* aggr = w.aggr + l * N * D2;
+    float* z1 = w.z1 + l * N * D2;
+    float* y1 = w.y1 + l * N * D2;
+    float* z2 = w.z2 + l * N * D;
+    const bool last = l == L - 1;
+    const PgnnDropout drop_in = drops.at(l > 0 ? l - 1 : 0), drop_out = drops.at(l);
+    // gather: columns 0..D the inputs (the previous layer's ReLU + dropout applied on load), D..2D the edge-encoder half S.T
+    const float* h = l == 0 ? w.h0 : w.z2 + (l - 1) * N * D;
+    TRY(pgnn_internal_aggregate_fwd(h, D, nullptr, nullptr, l > 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_SUM, nullptr, w.S, kBioQ,
+                                    w.T + l * kBioQ * D, nullptr, kBioQ, D, aggr, D2, st, nullptr, l > 0 ? &drop_in : nullptr));
+    // Linear 1; on the tensor path in training its epilogue also accumulates the inner BatchNorm's batch statistics
+    const float* gamma = (const float*)p[BG_GAMMA];
+    const float* beta = (const float*)p[BG_BETA];
+    float* rm = (float*)bn_running_mean[l];
+    float* rv = (float*)bn_running_var[l];
+    int64_t* nbt = bn_num_batches_tracked ? (int64_t*)bn_num_batches_tracked[l] : nullptr;
+    double* acc = w.bn_acc + l * 2 * D2;
+    bool stats_fused = false;
+    if (training && precision == 1) {
+      PGNN_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * 2 * D2, st));
+      PgnnGemmHooks hk;
+      hk.stats = acc;
+      const int rc = pgnn_tc_linear_fwd(aggr, D2, (const float*)p[BG_W1], (const float*)p[BG_B1], N, D2, D2, 0, z1, D2, st, &hk);
+      if (rc == PGNN_OK) stats_fused = true;
+      else if (rc != PGNN_EUNSUPPORTED) return rc;
+    }
+    if (!stats_fused) TRY(pgnn_linear_fwd(aggr, D2, (const float*)p[BG_W1], (const float*)p[BG_B1], N, D2, D2, 0, z1, D2, precision, st));
+    // inner BatchNorm1d(2D) + ReLU
+    if (stats_fused) {
+      PgnnBnFold fold{};
+      fold.acc = acc; fold.gamma = gamma; fold.beta = beta;
+      fold.running_mean = rm; fold.running_var = rv; fold.nbt = nbt;
+      fold.save_mean = w.mean + l * D2; fold.save_invstd = w.invstd + l * D2;
+      fold.momentum = momentum; fold.eps = eps; fold.set_rows((int)N);
+      TRY(pgnn_internal_bn_apply_fold(z1, D2, N, D2, fold, 1, y1, D2, st, nullptr));
+    } else if (training) {
+      TRY(pgnn_internal_bn_fwd_train(z1, D2, N, D2, gamma, beta, rm, rv, nbt, momentum, eps, 1, y1, D2, w.mean + l * D2, w.invstd + l * D2,
+                                     nullptr, nullptr, w.scratch, w.scratch_bytes, st, nullptr));
+    } else {
+      TRY(pgnn_bn_fwd_eval(z1, D2, N, D2, gamma, beta, rm, rv, eps, 1, y1, D2, st));
+    }
+    // Linear 2: the layer's pre-activation; the last layer without dropout writes node_rep itself
+    const bool direct = last && drop_out.p == 0.f;
+    TRY(pgnn_linear_fwd(y1, D2, (const float*)p[BG_W2], (const float*)p[BG_B2], N, D, D2, 0, direct ? node_rep : z2, direct ? ld_out : D,
+                        precision, st));
+    if (last && !direct) TRY(bio_act(false, z2, D, nullptr, 0, N, D, 0, drop_out, node_rep, ld_out, st));
+  }
+  return PGNN_OK;
+}
+
+int bio_gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg, const float* x, int64_t N, int64_t L, int64_t D,
+                     const Drops& drops, int precision, float* grads, const int64_t* off, const BioGinWs& w, cudaStream_t st) {
+  const int64_t D2 = 2 * D;
+  SideCtx* sc = precision == 1 ? side_ctx(st) : nullptr;
+  PGNN_CUDA(cudaMemsetAsync(w.gT, 0, sizeof(float) * L * kBioQ * D, st));
+  const float* gy = g_node_rep;
+  int64_t ldgy = ldg;
+  for (int64_t l = L - 1; l >= 0; --l) {
+    const void* const* p = params + PB_LAYER0 + l * BG_COUNT;
+    const int64_t* o = off + PB_LAYER0 + l * BG_COUNT;
+    const bool last = l == L - 1;
+    const int par = (int)(l & 1);
+    const float* aggr = w.aggr + l * N * D2;
+    const float* z1 = w.z1 + l * N * D2;
+    const float* y1 = w.y1 + l * N * D2;
+    float* gz2 = w.gz2 + (sc ? par * N * D : 0);
+    float* gz1 = w.gz1 + (sc ? par * N * D2 : 0);
+    // the gradient at the layer's pre-activation: its ReLU (inner layers) and dropout masks in one sweep
+    if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad has finished reading this copy
+    const float* gz;
+    int64_t ldgz;
+    TRY(bio_act_bwd(gz, ldgz, gy, ldgy, w.z2 + l * N * D, N, D, last, drops.at(l), gz2, st));
+    // Linear 2: weight and bias gradients (side stream), then the gradient of the BatchNorm's output
+    TRY(side_wgrad(sc, st, 0, par, precision, gz, ldgz, y1, D2, N, D, D2, grads + o[BG_W2], grads + o[BG_B2], w.wpart, w.wpart_floats));
+    TRY(pgnn_linear_bwd_x(gz, ldgz, (const float*)p[BG_W2], N, D, D2, nullptr, 0, w.gy1, D2, precision, st));
+    // inner BatchNorm + ReLU (mask recomputed from z1); the same pass leaves colsum(gz1) = the gradient of mlp.0.bias
+    if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[1][par], 0));
+    TRY(pgnn_internal_bn_bwd(w.gy1, D2, z1, D2, N, D2, (const float*)p[BG_GAMMA], (const float*)p[BG_BETA], w.mean + l * D2,
+                             w.invstd + l * D2, 1, gz1, D2, grads + o[BG_GAMMA], grads + o[BG_BETA], grads + o[BG_B1], w.scratch,
+                             w.scratch_bytes, st, nullptr));
+    // Linear 1
+    TRY(side_wgrad(sc, st, 1, par, precision, gz1, D2, aggr, D2, N, D2, D2, grads + o[BG_W1], nullptr, w.wpart, w.wpart_floats));
+    TRY(pgnn_linear_bwd_x(gz1, D2, (const float*)p[BG_W1], N, D2, D2, nullptr, 0, w.ga, D2, precision, st));
+    // the gather: gT_l = S^T ga[:, D:2D]; the node half goes back over the transpose graph
+    TRY(pgnn_internal_edge_table_bwd2(w.S, kBioQ, w.ga, D2, D, N, (int)D, w.gT + l * kBioQ * D, D, nullptr, kBioQ, st));
+    TRY(pgnn_aggregate_bwd(w.ga, D2, N, D, w.rowptr_s, w.nbr_s, PGNN_AGG_SUM, nullptr, w.rowptr_t, w.gh, D, st));
+    gy = w.gh;
+    ldgy = D;
+  }
+  return bio_backward_tail(kGin, sc, w.gT, w.gh, x, N, L, D, grads, off, st);
+}
+
+int bio_conv_forward(int type, const void* const* params, const float* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D,
+                     const Drops& drops, int precision, float* node_rep, int64_t ld_out, const BioConvWs& w, cudaStream_t st) {
+  const bool gat = type == PGNN_CONV_GAT;
+  const int64_t C = bio_width(type, D);
+  const int PL = bio_layer_params(type);
+  const float* h = w.h0;
+  for (int64_t l = 0; l < L; ++l) {
+    const void* const* p = params + PB_LAYER0 + l * PL;
+    const bool last = l == L - 1;
+    const PgnnDropout drop = drops.at(l);
+    float* xl = w.xl + l * N * C;
+    float* z = w.z + l * N * D;
+    const float* T = w.T + l * kBioQ * C;
+    // the last layer without dropout writes node_rep itself, except GraphSAGE, whose backward reads its normalised rows
+    const bool direct = last && drop.p == 0.f && type != PGNN_CONV_SAGE && ld_out % 4 == 0 && aligned16(node_rep);
+    float* out = direct ? node_rep : z;
+    const int64_t ldo = direct ? ld_out : D;
+    TRY(pgnn_linear_fwd(h, D, (const float*)p[gat ? BA_W : BC_W], (const float*)p[gat ? BA_B : BC_B], N, C, D, 0, xl, C, precision, st));
+    if (gat) {
+      TRY(pgnn_gat_fwd(xl, N, kHeads, D, (const float*)p[BA_ATT], T, 1, edge_attr, w.rowptr_t, w.nbr_t, w.eid_t, E, (const float*)p[BA_BIAS],
+                       kSlope, w.alpha + l * (E + N) * kHeads, w.pq + l * N * kHeads * 2, out, ldo, st));
+    } else if (type == PGNN_CONV_GCN) {
+      TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_GCN, w.dinv, w.S, kBioQ, T, nullptr,
+                                      kBioQ, 0, out, ldo, st, nullptr, nullptr));
+    } else {
+      // mean aggregation into the backward scratch `gz` (only its normalised rows and their norms are needed later)
+      TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_MEAN, nullptr, w.S, kBioQ, T, nullptr,
+                                      kBioQ, 0, w.gz, D, st, nullptr, nullptr));
+      TRY(pgnn_l2norm_fwd(w.gz, D, N, D, z, D, w.nrm + l * N, st));
+    }
+    float* hout = w.hout + l * N * D;
+    if (!last) TRY(bio_act(false, z, D, nullptr, 0, N, D, 1, drop, hout, D, st));
+    else if (!direct) TRY(bio_act(false, z, D, nullptr, 0, N, D, 0, drop, node_rep, ld_out, st));
+    h = hout;
+  }
+  return PGNN_OK;
+}
+
+int bio_conv_backward(int type, const void* const* params, const float* g_node_rep, int64_t ldg, const float* x, const float* edge_attr,
+                      int64_t N, int64_t E, int64_t L, int64_t D, const Drops& drops, int precision, float* grads, const int64_t* off,
+                      const BioConvWs& w, cudaStream_t st) {
+  const bool gat = type == PGNN_CONV_GAT;
+  const int64_t C = bio_width(type, D);
+  const int PL = bio_layer_params(type);
+  SideCtx* sc = precision == 1 ? side_ctx(st) : nullptr;
+  if (!gat) PGNN_CUDA(cudaMemsetAsync(w.gT, 0, sizeof(float) * L * kBioQ * C, st));  // GAT's backward overwrites its table gradient
+  const float* gy = g_node_rep;
+  int64_t ldgy = ldg;
+  for (int64_t l = L - 1; l >= 0; --l) {
+    const void* const* p = params + PB_LAYER0 + l * PL;
+    const int64_t* o = off + PB_LAYER0 + l * PL;
+    const bool last = l == L - 1;
+    const int par = (int)(l & 1);
+    const float* xl = w.xl + l * N * C;
+    const float* z = w.z + l * N * D;
+    const float* hin = l == 0 ? w.h0 : w.hout + (l - 1) * N * D;
+    float* gxl = w.gxl + (sc ? par * N * C : 0);
+    float* gT = w.gT + l * kBioQ * C;
+    const float* gz;
+    int64_t ldgz;
+    TRY(bio_act_bwd(gz, ldgz, gy, ldgy, z, N, D, last, drops.at(l), w.gz, st));
+    if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad has finished reading this copy of gxl
+    if (gat) {
+      TRY(pgnn_gat_bwd(gz, ldgz, xl, N, kHeads, D, (const float*)p[BA_ATT], w.T + l * kBioQ * C, 1, edge_attr, w.rowptr_t, w.nbr_t, w.eid_t,
+                       w.rowptr_s, w.nbr_s, w.eid_s, E, kSlope, w.alpha + l * (E + N) * kHeads, w.pq + l * N * kHeads * 2, gxl,
+                       grads + o[BA_ATT], gT, grads + o[BA_BIAS], w.scratch, w.scratch_bytes, st));
+    } else {
+      const float* ga = gz;
+      int64_t ldga = ldgz;
+      if (type == PGNN_CONV_SAGE) {
+        TRY(pgnn_l2norm_bwd(gz, ldgz, z, D, w.nrm + l * N, N, D, w.ga, D, st));
+        ga = w.ga;
+        ldga = D;
+      }
+      TRY(pgnn_internal_edge_table_bwd2(w.S, kBioQ, ga, ldga, 0, N, (int)D, gT, D, nullptr, kBioQ, st));
+      TRY(pgnn_aggregate_bwd(ga, ldga, N, D, w.rowptr_s, w.nbr_s, agg_mode(type), w.dinv, w.rowptr_t, gxl, D, st));
+    }
+    // Linear: weight + bias gradients (side stream), then the input gradient
+    TRY(side_wgrad(sc, st, 0, par, precision, gxl, C, hin, D, N, C, D, grads + o[gat ? BA_W : BC_W], grads + o[gat ? BA_B : BC_B], w.wpart,
+                   w.wpart_floats));
+    TRY(pgnn_linear_bwd_x(gxl, C, (const float*)p[gat ? BA_W : BC_W], N, C, D, nullptr, 0, w.gh, D, precision, st));
+    gy = w.gh;
+    ldgy = D;
+  }
+  return bio_backward_tail(type, sc, w.gT, w.gh, x, N, L, D, grads, off, st);
+}
+
 }  // namespace
 
 extern "C" {
@@ -774,6 +1264,74 @@ int pgnn_chem_encoder_backward(int gnn_type, const void* const* params, const fl
     return gin_backward(params, g_node_rep, ldg, x, N, E, L, D, drops, precision, grads, workspace, workspace_bytes, stream);
   return conv_backward(gnn_type, params, g_node_rep, ldg, x, edge_attr, N, E, L, D, drops, precision, grads, workspace, workspace_bytes,
                        stream);
+}
+
+// ------------------------------------------------------------------------------------------------------------------------------
+// bio, every type, with dropout
+// ------------------------------------------------------------------------------------------------------------------------------
+int64_t pgnn_bio_encoder_num_params(int gnn_type, int64_t L) {
+  if (!valid_type(gnn_type) || L < 1) return PGNN_EINVAL;
+  return bio_grad_layout(gnn_type, L, 0, nullptr);
+}
+
+int pgnn_bio_encoder_grad_offsets(int gnn_type, int64_t L, int64_t D, int64_t* offsets) {
+  PGNN_CHECK_ARG(valid_type(gnn_type) && L >= 1 && D > 0 && offsets);
+  bio_grad_layout(gnn_type, L, D, offsets);
+  return PGNN_OK;
+}
+
+int64_t pgnn_bio_encoder_workspace_bytes(int gnn_type, int64_t N, int64_t E, int64_t L, int64_t D) {
+  if (!valid_type(gnn_type) || N < 0 || E < 0 || L < 1 || D <= 0) return PGNN_EINVAL;
+  return bio_workspace_bytes(gnn_type, N, E, L, D);
+}
+
+int pgnn_bio_encoder_forward(int gnn_type, const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
+                             void* const* bn_num_batches_tracked, const float* x, const int64_t* edge_index, const float* edge_attr,
+                             int64_t N, int64_t E, int64_t L, int64_t D, int training, float momentum, float eps, float drop_p,
+                             int64_t drop_seed, int precision, float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes,
+                             void* stream) {
+  PGNN_CHECK_ARG(valid_type(gnn_type) && drop_p >= 0.f && drop_p <= 1.f);
+  PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && workspace);
+  PGNN_CHECK_ARG(gnn_type != kGin || (bn_running_mean && bn_running_var));
+  PGNN_CHECK_ARG(N == 0 || (x && node_rep && ld_out >= D));
+  PGNN_CHECK_ARG(E == 0 || (edge_index && edge_attr));
+  if (workspace_bytes < bio_workspace_bytes(gnn_type, N, E, L, D)) return PGNN_EWORKSPACE;
+  if (N == 0) return PGNN_OK;
+  Drops drops;
+  if (training) drops = Drops{drop_p, drop_seed};  // eval mode has no dropout
+  cudaStream_t st = as_stream(stream);
+  if (gnn_type == kGin) {
+    const BioGinWs w = carve_bio_gin(workspace, N, E, L, D);
+    TRY(bio_prologue(kGin, w, w.T, params, x, edge_index, edge_attr, N, E, L, D, w.scratch, w.scratch_bytes, st));
+    return bio_gin_forward(params, bn_running_mean, bn_running_var, bn_num_batches_tracked, N, L, D, training, momentum, eps, drops,
+                           precision, node_rep, ld_out, w, st);
+  }
+  const BioConvWs w = carve_bio_conv(workspace, gnn_type, N, E, L, D);
+  TRY(bio_prologue(gnn_type, w, w.T, params, x, edge_index, edge_attr, N, E, L, D, w.scratch, w.scratch_bytes, st));
+  return bio_conv_forward(gnn_type, params, edge_attr, N, E, L, D, drops, precision, node_rep, ld_out, w, st);
+}
+
+int pgnn_bio_encoder_backward(int gnn_type, const void* const* params, const float* g_node_rep, int64_t ldg, const float* x,
+                              const float* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, float drop_p, int64_t drop_seed,
+                              int precision, float* grads, void* workspace, int64_t workspace_bytes, void* stream) {
+  PGNN_CHECK_ARG(valid_type(gnn_type) && drop_p >= 0.f && drop_p <= 1.f);
+  PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && grads && workspace);
+  if (workspace_bytes < bio_workspace_bytes(gnn_type, N, E, L, D)) return PGNN_EWORKSPACE;
+  const int64_t count = bio_grad_layout(gnn_type, L, D, nullptr);
+  std::vector<int64_t> offsets(count + 1);
+  bio_grad_layout(gnn_type, L, D, offsets.data());
+  cudaStream_t st = as_stream(stream);
+  if (N == 0) {
+    PGNN_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * offsets[count], st));
+    return PGNN_OK;
+  }
+  PGNN_CHECK_ARG(g_node_rep && x && ldg >= D && (E == 0 || gnn_type != PGNN_CONV_GAT || edge_attr));
+  const Drops drops{drop_p, drop_seed};
+  if (gnn_type == kGin)
+    return bio_gin_backward(params, g_node_rep, ldg, x, N, L, D, drops, precision, grads, offsets.data(),
+                            carve_bio_gin(workspace, N, E, L, D), st);
+  return bio_conv_backward(gnn_type, params, g_node_rep, ldg, x, edge_attr, N, E, L, D, drops, precision, grads, offsets.data(),
+                           carve_bio_conv(workspace, gnn_type, N, E, L, D), st);
 }
 
 }  // extern "C"

@@ -285,8 +285,8 @@ class GradAllReducer:
 
 
 def encoder_flat_source(gnn):
-    """flat_sources entry for a chem GNN running the fused path: (last flat gradient buffer, its parameters).
-    `bind(buffer)` makes the encoder's backward write its gradients into `buffer` (see ChemEncoderPlan.grad_buffer)."""
+    """flat_sources entry for a chem or bio GNN running the fused path: (last flat gradient buffer, its parameters).
+    `bind(buffer)` makes the encoder's backward write its gradients into `buffer` (see ops._EncoderPlan.grad_buffer)."""
     def src():
         plan = gnn._fused_plan()
         if plan is None:

@@ -679,7 +679,7 @@ def gat(xl, att, T, edge_attr, graph, bias, heads=2, slope=0.2, is_bio=False):
 
 
 # ------------------------------------------------------------------------------------------------
-# whole-encoder fast path: chem GIN / GCN / GraphSAGE / GAT with dropout (pgnn_chem_encoder_*)
+# whole-encoder fast path: chem and bio GIN / GCN / GraphSAGE / GAT with dropout (pgnn_chem_encoder_*, pgnn_bio_encoder_*)
 # ------------------------------------------------------------------------------------------------
 import ctypes as _ct
 
@@ -687,7 +687,7 @@ CONV_TYPE = {"gcn": 1, "graphsage": 2, "gat": 3}
 
 
 def _layer_params(gnn_type, conv):
-    """One conv's parameters in the order of include/pgnn_b200.h (also the flat gradient order)."""
+    """One chem conv's parameters in the order of include/pgnn_b200.h (also the flat gradient order)."""
     if gnn_type == "gin":
         ps = [conv.mlp[0].weight, conv.mlp[0].bias, conv.mlp[2].weight, conv.mlp[2].bias]
     elif gnn_type == "gat":
@@ -697,38 +697,39 @@ def _layer_params(gnn_type, conv):
     return ps + [conv.edge_embedding1.weight, conv.edge_embedding2.weight]
 
 
-class ChemEncoderPlan:
-    """Per-module bookkeeping for the whole-encoder chem GNN: parameter order, gradient layout, pointer tables, and the C calls.
-    Every type runs on pgnn_chem_encoder_* (type code 0 = GIN, else PGNN_CONV_*); GIN's layout queries are pgnn_chem_gin_*, the
-    conv types' pgnn_chem_conv_*.  The plan's methods are the only code that tells them apart."""
+def _bio_layer_params(gnn_type, conv):
+    """One bio conv's parameters in the order of include/pgnn_b200.h (pgnn_bio_encoder_*)."""
+    if gnn_type == "gin":
+        ps = [conv.mlp[0].weight, conv.mlp[0].bias, conv.mlp[1].weight, conv.mlp[1].bias, conv.mlp[3].weight, conv.mlp[3].bias]
+    elif gnn_type == "gat":
+        ps = [conv.weight_linear.weight, conv.weight_linear.bias, conv.att, conv.bias]
+    else:
+        ps = [conv.linear.weight, conv.linear.bias]
+    return ps + [conv.edge_encoder.weight, conv.edge_encoder.bias]
 
-    def __init__(self, gnn, gnn_type):
+
+class _EncoderPlan:
+    """Per-module bookkeeping of a whole-encoder GNN: parameter order, gradient layout, pointer tables, and the C calls.  The
+    domain's subclass collects the parameters and BatchNorm modules, checks the inputs and makes the C calls; everything else is
+    shared."""
+    domain = None
+
+    def _setup(self, gnn_type, L, D, params, bns, offsets):
         self.gnn_type = gnn_type
         self.conv = 0 if gnn_type == "gin" else CONV_TYPE[gnn_type]
-        self.L = len(gnn.gnns)
-        self.D = gnn.x_embedding1.weight.shape[1]
-        ps = [gnn.x_embedding1.weight, gnn.x_embedding2.weight]
-        for conv, bn in zip(gnn.gnns, gnn.batch_norms):
-            ps += _layer_params(gnn_type, conv) + [bn.weight, bn.bias]
-        self.params = ps
-        n = len(ps)
-        off = (_ct.c_int64 * (n + 1))()
-        if self.conv:
-            assert n == lib.pgnn_chem_conv_num_params(self.conv, self.L)
-            check(lib.pgnn_chem_conv_grad_offsets(self.conv, self.L, self.D, off), "chem_conv_grad_offsets")
-        else:
-            assert n == lib.pgnn_chem_gin_num_params(self.L)
-            check(lib.pgnn_chem_gin_grad_offsets(self.L, self.D, off), "chem_gin_grad_offsets")
-        self.offsets = list(off)
+        self.L, self.D = L, D
+        self.params = params
+        n = len(params)
+        self.offsets = list(offsets)
         self.sizes = [self.offsets[i + 1] - self.offsets[i] for i in range(n)]
-        self.shapes = [tuple(p.shape) for p in ps]
-        for p, s in zip(ps, self.sizes):
+        self.shapes = [tuple(p.shape) for p in params]
+        for p, s in zip(params, self.sizes):
             if p.numel() != s:
-                raise PgnnError("parameter shape does not match the chem %s layout (emb_dim / heads / vocabulary sizes)" % gnn_type)
+                raise PgnnError("parameter shape does not match the %s %s layout (emb_dim / heads / vocabulary sizes)" % (self.domain, gnn_type))
         self.total = self.offsets[-1]
         self.PtrArr = _ct.c_void_p * n
-        self.BnArr = _ct.c_void_p * self.L
-        self.bns = list(gnn.batch_norms)
+        self.BnArr = _ct.c_void_p * L
+        self.bns = bns              # the BatchNorm1d modules whose state the encoder updates: one per layer, or none
         self._ws_alloc = 0          # workspace bytes requested from the allocator so far (see workspace_bytes)
         self.last_flat_grad = None  # the flat gradient buffer of the most recent backward (all-reduce target)
         # optional caller-owned destination ([total] fp32, e.g. a slice of NVLink-symmetric memory): used instead of a fresh
@@ -750,15 +751,62 @@ class ChemEncoderPlan:
         Batches differ by a few percent in N and E; asking for exactly the need makes every new maximum a cudaMalloc
         (milliseconds, and a device synchronisation) in the middle of training, whereas one size per plan is served from the
         caching allocator's free list."""
-        if self.conv:
-            need = lib.pgnn_chem_conv_workspace_bytes(self.conv, N, E, self.L, self.D)
-        else:
-            need = lib.pgnn_chem_gin_workspace_bytes(N, E, self.L, self.D)
+        need = self._need(N, E)
         if need < 0:
             return need
         if need > self._ws_alloc:
             self._ws_alloc = ((need + need // 16) + (16 << 20) - 1) // (16 << 20) * (16 << 20)
         return self._ws_alloc
+
+    def bn_pointers(self):
+        """(running_mean, running_var, num_batches_tracked) host pointer tables of the L BatchNorms, or Nones without any."""
+        if not self.bns:
+            return None, None, None
+        return tuple(self.BnArr(*[getattr(b, k).data_ptr() for b in self.bns]) for k in ("running_mean", "running_var", "num_batches_tracked"))
+
+    def bn_constants(self):
+        """(momentum, eps) the BatchNorms run with (torch's defaults for an encoder without BatchNorm)."""
+        if not self.bns:
+            return 0.1, 1e-5
+        b = self.bns[0]
+        return (b.momentum if b.momentum is not None else 0.1), b.eps
+
+
+class ChemEncoderPlan(_EncoderPlan):
+    """The chem GNN on pgnn_chem_encoder_* (type code 0 = GIN, else PGNN_CONV_*); GIN's layout queries are pgnn_chem_gin_*, the
+    conv types' pgnn_chem_conv_*."""
+    domain = "chem"
+
+    def __init__(self, gnn, gnn_type):
+        L, D = len(gnn.gnns), gnn.x_embedding1.weight.shape[1]
+        ps = [gnn.x_embedding1.weight, gnn.x_embedding2.weight]
+        for conv, bn in zip(gnn.gnns, gnn.batch_norms):
+            ps += _layer_params(gnn_type, conv) + [bn.weight, bn.bias]
+        n = len(ps)
+        off = (_ct.c_int64 * (n + 1))()
+        if gnn_type != "gin":
+            assert n == lib.pgnn_chem_conv_num_params(CONV_TYPE[gnn_type], L)
+            check(lib.pgnn_chem_conv_grad_offsets(CONV_TYPE[gnn_type], L, D, off), "chem_conv_grad_offsets")
+        else:
+            assert n == lib.pgnn_chem_gin_num_params(L)
+            check(lib.pgnn_chem_gin_grad_offsets(L, D, off), "chem_gin_grad_offsets")
+        self._setup(gnn_type, L, D, ps, list(gnn.batch_norms), off)
+
+    def _need(self, N, E):
+        if self.conv:
+            return lib.pgnn_chem_conv_workspace_bytes(self.conv, N, E, self.L, self.D)
+        return lib.pgnn_chem_gin_workspace_bytes(N, E, self.L, self.D)
+
+    @staticmethod
+    def inputs(x, edge_index, edge_attr):
+        if x.dtype != torch.int64 or x.dim() != 2 or x.shape[1] != 2:
+            raise PgnnError("chem node features must be int64 [N, 2]")
+        if edge_index.dtype != torch.int64 or edge_index.dim() != 2 or edge_index.shape[0] != 2:
+            raise PgnnError("edge_index must be int64 [2, E]")
+        x, ei, ea = x.contiguous(), edge_index.contiguous(), edge_attr.contiguous()
+        if ea.dtype != torch.int64 or tuple(ea.shape) != (ei.shape[1], 2):
+            raise PgnnError("chem edge_attr must be int64 [E, 2]")
+        return x, ei, ea
 
     def forward(self, ptrs, rm, rv, nbt, x, ei, ea, N, E, training, momentum, eps, drop_p, drop_seed, precision, out, ws, wsb):
         check(lib.pgnn_chem_encoder_forward(self.conv, ptrs, rm, rv, nbt, _p(x), _p(ei), _p(ea), N, E, self.L, self.D, int(training),
@@ -770,6 +818,48 @@ class ChemEncoderPlan:
         also the one-hot atom-code rows, which only a tf32x3 training forward writes)."""
         check(lib.pgnn_chem_encoder_backward(self.conv, ptrs, _p(g), g.stride(0), _p(x), _p(ea), N, E, self.L, self.D, float(drop_p),
                                              int(drop_seed), precision, _p(flat), _p(ws), wsb, _st()), "chem_encoder_backward")
+
+
+class BioEncoderPlan(_EncoderPlan):
+    """The bio GNN on pgnn_bio_encoder_* (type code 0 = GIN, else PGNN_CONV_*).  Only GIN has BatchNorm state: the inner
+    BatchNorm1d(2D) of each layer's MLP."""
+    domain = "bio"
+
+    def __init__(self, gnn, gnn_type):
+        L, D = len(gnn.gnns), gnn.gnns[0].input_node_embeddings.weight.shape[1]
+        ps = [gnn.gnns[0].input_node_embeddings.weight]
+        for conv in gnn.gnns:
+            ps += _bio_layer_params(gnn_type, conv)
+        code = 0 if gnn_type == "gin" else CONV_TYPE[gnn_type]
+        n = len(ps)
+        assert n == lib.pgnn_bio_encoder_num_params(code, L)
+        off = (_ct.c_int64 * (n + 1))()
+        check(lib.pgnn_bio_encoder_grad_offsets(code, L, D, off), "bio_encoder_grad_offsets")
+        self._setup(gnn_type, L, D, ps, [conv.mlp[1] for conv in gnn.gnns] if gnn_type == "gin" else [], off)
+
+    def _need(self, N, E):
+        return lib.pgnn_bio_encoder_workspace_bytes(self.conv, N, E, self.L, self.D)
+
+    @staticmethod
+    def inputs(x, edge_index, edge_attr):
+        """x: the dummy node label, [N] or [N, 1] (any dtype, taken as float32 as the layer-by-layer embedding does)."""
+        if x.dim() not in (1, 2) or (x.dim() == 2 and x.shape[1] != 1):
+            raise PgnnError("bio node labels must be [N] or [N, 1]")
+        if edge_index.dtype != torch.int64 or edge_index.dim() != 2 or edge_index.shape[0] != 2:
+            raise PgnnError("edge_index must be int64 [2, E]")
+        x, ei, ea = x.reshape(-1).to(torch.float32).contiguous(), edge_index.contiguous(), edge_attr.contiguous()
+        if ea.dtype != torch.float32 or tuple(ea.shape) != (ei.shape[1], 9):
+            raise PgnnError("bio edge_attr must be float32 [E, 9]")
+        return x, ei, ea
+
+    def forward(self, ptrs, rm, rv, nbt, x, ei, ea, N, E, training, momentum, eps, drop_p, drop_seed, precision, out, ws, wsb):
+        check(lib.pgnn_bio_encoder_forward(self.conv, ptrs, rm, rv, nbt, _p(x), _p(ei), _p(ea), N, E, self.L, self.D, int(training),
+                                           float(momentum), float(eps), float(drop_p), int(drop_seed), precision, _p(out), self.D,
+                                           _p(ws), wsb, _st()), "bio_encoder_forward")
+
+    def backward(self, ptrs, g, x, ea, N, E, drop_p, drop_seed, precision, flat, ws, wsb):
+        check(lib.pgnn_bio_encoder_backward(self.conv, ptrs, _p(g), g.stride(0), _p(x), _p(ea), N, E, self.L, self.D, float(drop_p),
+                                            int(drop_seed), precision, _p(flat), _p(ws), wsb, _st()), "bio_encoder_backward")
 
 
 def _deliver_flat_grads(plan, ctx, run):
@@ -821,38 +911,32 @@ def _release_ctx(ctx):
     ctx.released = True
 
 
-_ENC_ARGS = 7  # _ChemEncoder.forward's arguments in front of the parameters
+_ENC_ARGS = 7  # _Encoder.forward's arguments in front of the parameters
 
 
-class _ChemEncoder(Function):
+class _Encoder(Function):
+    """The whole encoder of either domain as one autograd node; the plan (ChemEncoderPlan / BioEncoderPlan) checks the inputs and
+    makes the two C calls."""
+
     @staticmethod
     def forward(ctx, plan, x, edge_index, edge_attr, training, drop_p, drop_seed, *params):
         _dev(x, edge_index, edge_attr, *params)
-        if x.dtype != torch.int64 or x.dim() != 2 or x.shape[1] != 2:
-            raise PgnnError("chem node features must be int64 [N, 2]")
-        if edge_index.dtype != torch.int64 or edge_index.dim() != 2 or edge_index.shape[0] != 2:
-            raise PgnnError("edge_index must be int64 [2, E]")
-        x, ei, ea = x.contiguous(), edge_index.contiguous(), edge_attr.contiguous()
+        x, ei, ea = plan.inputs(x, edge_index, edge_attr)
         N, E, D = x.shape[0], ei.shape[1], plan.D
-        if ea.dtype != torch.int64 or tuple(ea.shape) != (E, 2):
-            raise PgnnError("chem edge_attr must be int64 [E, 2]")
         for p in params:
             if p.dtype != torch.float32 or not p.is_contiguous():
                 raise PgnnError("the fused encoder needs contiguous fp32 parameters")
-        if training and N == 0:
+        if training and N == 0 and plan.bns:
             raise PgnnError("BatchNorm in training mode needs at least one node")
         dev = x.device
         ptrs = plan.PtrArr(*[p.data_ptr() for p in params])
-        bns = plan.bns
-        rm = plan.BnArr(*[b.running_mean.data_ptr() for b in bns])
-        rv = plan.BnArr(*[b.running_var.data_ptr() for b in bns])
-        nbt = plan.BnArr(*[b.num_batches_tracked.data_ptr() for b in bns])
+        rm, rv, nbt = plan.bn_pointers()
         wsb = plan.workspace_bytes(N, E)
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
         out = torch.empty(N, D, dtype=torch.float32, device=dev)
-        mom = bns[0].momentum if bns[0].momentum is not None else 0.1
+        mom, eps = plan.bn_constants()
         precision = _precision
-        plan.forward(ptrs, rm, rv, nbt, x, ei, ea, N, E, training, mom, bns[0].eps, drop_p, drop_seed, precision, out, ws, wsb)
+        plan.forward(ptrs, rm, rv, nbt, x, ei, ea, N, E, training, mom, eps, drop_p, drop_seed, precision, out, ws, wsb)
         ctx.plan, ctx.ws, ctx.wsb, ctx.ptrs, ctx.x, ctx.ea, ctx.dims, ctx.training = plan, ws, wsb, ptrs, x, ea, (N, E), training
         ctx.drop = (drop_p, drop_seed)  # the backward regenerates the masks from these
         ctx.precision = precision       # and reads the workspace this precision's forward wrote, whatever set_precision says by then
@@ -884,13 +968,18 @@ class _ChemEncoder(Function):
 def chem_encoder(plan: ChemEncoderPlan, x, edge_index, edge_attr, training: bool, drop_p: float = 0.0, drop_seed: int = 0):
     """The whole chem encoder in one call per pass.  With training and drop_p > 0, layer l's output carries the ops.dropout mask
     of (drop_p, drop_seed, l): the same mask the layer-by-layer composition applies under the same seed."""
-    return _ChemEncoder.apply(plan, x, edge_index, edge_attr, training, float(drop_p), int(drop_seed), *plan.params)
+    return _Encoder.apply(plan, x, edge_index, edge_attr, training, float(drop_p), int(drop_seed), *plan.params)
+
+
+def bio_encoder(plan: BioEncoderPlan, x, edge_index, edge_attr, training: bool, drop_p: float = 0.0, drop_seed: int = 0):
+    """The whole bio encoder in one call per pass, with the dropout masks of chem_encoder."""
+    return _Encoder.apply(plan, x, edge_index, edge_attr, training, float(drop_p), int(drop_seed), *plan.params)
 
 
 def chem_gin_relu_masks(plan: ChemEncoderPlan, gnn):
     """The ReLU decisions of the last training forward of the fused GIN encoder (plan.keep_workspace = True), in the order the
     reference takes them: per layer the MLP's hidden units [N, 2D], then (all but the last layer) the post-BatchNorm units [N, D]."""
-    if plan.gnn_type != "gin":
+    if plan.gnn_type != "gin" or plan.domain != "chem":
         raise PgnnError("chem_gin_relu_masks reads the GIN workspace layout (pgnn_chem_gin_debug_layout)")
     ws, (N, E, L, D) = plan.last_ws
     off = (_ct.c_int64 * 4)()
