@@ -384,6 +384,22 @@ PGNN_API int pgnn_debug_tc_wgrad(const float* gy, int64_t ldgy, const float* x, 
 PGNN_API int pgnn_debug_tc_wgrad_plan(int64_t M, int64_t N, int64_t K, int64_t* out4);
 PGNN_API int pgnn_debug_transpose_batch(int count, const float* const* in, float* const* out, const int32_t* rows,
                                         const int32_t* cols, void* stream);
+/* test aids for the weight-image path of the same GEMM (the forward and dgrad GEMMs of the chem GIN encoder): a weight used as a
+ * reduction-contiguous B [rows, K] is split into tf32 hi / lo once and stored as two planes, hi then lo, each
+ * [ceil(rows / 128) * 128][ceil(K / 32) * 32] floats row-major (image floats = 2 x that); inside every 32-wide block of a row, slot
+ * s holds element k = kperm(s) = (s & 16) | ((s & 3) << 2) | ((s >> 2) & 3) of the block; padding is zero.  hi = x + 0 with its low
+ * 13 bits cleared, lo = x - hi (fp32).
+ *   pgnn_debug_pack_weight_images: count <= 32 images in one launch (HOST arrays): job i reads w[i] [rows[i], cols[i]] with row
+ *     stride ld[i] >= cols[i] and writes into img[i] (16-byte aligned) the image of w[i] (transposed[i] == 0: B rows = rows[i],
+ *     K = cols[i]) or of its transpose (B rows = cols[i], K = rows[i]).  PGNN_EUNSUPPORTED above 32 jobs.
+ *   pgnn_debug_tc_gemm_img: pgnn_debug_tc_gemm with a_kc = b_kc = 1 (same arguments and epilogue, bit for bit the same result)
+ *     through the image path: packs B [N, K] into img (16-byte aligned, image floats of N rows and K) and runs the GEMM from it. */
+PGNN_API int pgnn_debug_pack_weight_images(int count, const float* const* w, const int64_t* ld, const int32_t* rows,
+                                           const int32_t* cols, const int32_t* transposed, float* const* img, void* stream);
+PGNN_API int pgnn_debug_tc_gemm_img(int bn, const float* A, int64_t lda, const float* B, int64_t ldb, float* img, float* C,
+                                    int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias, int relu, const float* mask,
+                                    int64_t ldm, float* colsum, double* stats, const float* S, int Q, float* gT, float* gT2,
+                                    int q_split, int64_t ldt, void* stream);
 /* test aids for the two BatchNorm sweeps only the whole encoder reaches (dropout of (drop_p, drop_seed, drop_layer) as in
  * pgnn_dropout_fwd; drop_p = 0 runs the mask-free kernels):
  *   pgnn_debug_bn_apply_fold: pgnn_bn_fwd_train's finalisation and apply in one kernel, from raw fp64 sums[2][C] (sum, sum of

@@ -21,6 +21,9 @@
 //     along whichever extent is contiguous, zero-filled out of range) while the tensor cores work on block kb, then
 //     splits it into hi / lo and stores both, permuted like A, in the K-major 128B-swizzled layout (tf32 wgmma reads a
 //     K-major B only, so an MN-major source is transposed on this store), and fences the stores to the async proxy;
+//   * B_IMG (K-major A and B only): B is a weight, the same for the whole pass, so it is split and laid out once per pass into a
+//     pre-split image (see kperm below) and every stage is filled by cp.async 16-byte copies, two blocks ahead, in the commit
+//     group of an A copy: no registers, no split and no scalar stores in the mainloop, and no global load in front of a barrier;
 //   * per k-step and warpgroup: one commit group of 3 wgmma.m64nBNk8 (lo*hi, hi*lo into the cross-term accumulator,
 //     hi*hi into its own), A fragments in FRAG_SETS register sets.  A set is rewritten only after wait_group has
 //     retired the group that read it, so FRAG_SETS - 1 groups stay queued across k-steps, k-blocks and the one barrier
@@ -110,6 +113,15 @@ __device__ __forceinline__ void fence_acc(float (&d)[R]) {
 // swap (an involution, so it also maps a slot back to its k).  k-step j, fragment column c (thread t = c mod 4 of its quad)
 // then holds k = 16 (j / 2) + 4 t + 2 (j % 2) + c / 4: thread t's slots are k = 4t .. 4t + 3 and 16 + 4t .. 16 + 4t + 3.
 __device__ __forceinline__ int kperm(int k) { return (k & 16) | ((k & 3) << 2) | ((k >> 2) & 3); }
+
+// Weight image: a K-major B operand [rows][K] (the GEMM's N extent x its reduction) split once into two planes, hi then lo, each
+// [align_up(rows, 128)][align_up(K, 32)] floats, row-major.  Inside every 32-wide block of a row, slot kperm(k) holds element k
+// (split_tf32, as the mainloop would split it); padded rows and reduction columns are zero.  So the aligned 16-byte piece at
+// (r, 32 kb + 4 c) of a plane is the chunk sw128_off(r mod BN, 4 c) of block kb's stage of that plane: one cp.async16, no tail
+// handling, and the zeros are the ones ldg4_tail would have filled in.
+constexpr int kImgRows = 128;  // row padding: a whole BN = 64 or 128 tile is always inside the image
+__host__ __device__ constexpr int64_t img_rows(int64_t rows) { return (rows + kImgRows - 1) / kImgRows * kImgRows; }
+__host__ __device__ constexpr int64_t img_ld(int64_t k) { return (k + BK - 1) / BK * BK; }
 
 // float offset of element (m, k) of a raw MN-major A block [BK][BM].  The XOR keeps 4-row pieces contiguous and spreads both
 // the loader's 16-byte stores (k and k + 1) and the fragment reads (8 rows x 4 threads of a quad) over all 32 banks.
@@ -224,7 +236,7 @@ struct Loader {
 };
 
 // A: block kb of this CTA's 128 rows copied raw into a shared-memory buffer (akc_off / araw_off layout) with cp.async, so the
-// copy in flight holds no registers.  Same pieces as Loader<KC, BM>; out-of-range elements are zero-filled.
+// copy in flight holds no registers.  Same pieces as Loader<KC, BM>; out-of-range elements are zero-filled.  The caller commits.
 template <bool KC>
 __device__ __forceinline__ void a_copy(float* dst, const float* __restrict__ A, int64_t lda, int m0, int M, int k0, int krem) {
 #pragma unroll
@@ -238,25 +250,50 @@ __device__ __forceinline__ void a_copy(float* dst, const float* __restrict__ A, 
     const float* src = n > 0 ? (KC ? A + (int64_t)gr * lda + k0 + kk : A + (int64_t)(k0 + kk) * lda + gr) : A;
     cp_async16(dst + (KC ? akc_off(rr, kk) : araw_off(rr, kk)), src, 4 * n);
   }
-  cp_async_commit();
 }
 
-constexpr int NSTAGE = 3;  // B stages: block kb + 1 is stored while blocks kb - 1 and kb may still be read
-
+// B from a weight image: block kb of this CTA's BN rows (both planes, `plane` floats apart) into one stage with cp.async.  Thread
+// pieces as Loader<true, BN>: 8 threads cover one 128-byte row of a plane.  The caller commits.
 template <int BN>
+__device__ __forceinline__ void b_img_copy(uint8_t* hi, uint8_t* lo, const float* __restrict__ img, int64_t ld, int64_t plane, int n0,
+                                           int k0) {
+#pragma unroll
+  for (int i = 0; i < Loader<true, BN>::NV; ++i) {
+    const int f = threadIdx.x + i * NTHREADS, rr = f >> 3, kk = (f & 7) * 4;
+    const float* src = img + (int64_t)(n0 + rr) * ld + k0 + kk;
+    const int o = sw128_off(rr, kk);
+    cp_async16(reinterpret_cast<float*>(hi + o), src, 16);
+    cp_async16(reinterpret_cast<float*>(lo + o), src + plane, 16);
+  }
+}
+
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+constexpr int NSTAGE = 3;  // raw B stages: block kb + 1 is stored while blocks kb - 1 and kb may still be read
+
+template <int BN, bool B_IMG = false>
 struct TileCfg {
   static constexpr int B_BYTES = BN * BK * 4;
   static constexpr int STAGE = 2 * B_BYTES;      // [B hi | B lo]
-  static constexpr int A_RAW = BM * BK * 4;      // one raw A block (16 KiB), two buffers
+  static constexpr int A_RAW = BM * BK * 4;      // one raw A block (16 KiB)
+  // Copy distance in blocks.  Raw B: block kb + 1 is loaded and stored during block kb (NSTAGE stages), A one block ahead (two
+  // buffers).  Image B: two blocks ahead, so a copy has a whole block of MMAs more to land than the barrier in front of it needs;
+  // the stages hold blocks kb - 1 (still read by queued wgmma), kb, kb + 1 and kb + 2 (being copied).  A goes two ahead too where
+  // its third buffer fits: BN = 128, 4 x 32 KiB + 3 x 16 KiB = 176 KiB (one CTA per SM); at BN = 64, 4 x 16 KiB + 2 x 16 KiB =
+  // 96 KiB keeps two CTAs per SM (a third A buffer, 112 KiB + 1 KiB slack each, would not).
+  static constexpr int B_STAGES = B_IMG ? 4 : NSTAGE;
+  static constexpr int A_DIST = B_IMG && BN == 128 ? 2 : 1;
+  static constexpr int A_BUFS = A_DIST + 1;
   static constexpr int SLD = BN + 4;             // epilogue staging row stride (16-byte aligned rows)
   static constexpr int EPI = BM * SLD * 4 + BM * kMaxHookQ * 4;  // staging tile + the hooks' [128][Q <= 16] slice
-  static constexpr int RING = NSTAGE * STAGE + 2 * A_RAW;
+  static constexpr int RING = B_STAGES * STAGE + A_BUFS * A_RAW;
   static constexpr int SMEM = (RING > EPI ? RING : EPI) + 1024;  // + alignment slack of the 1024-byte swizzle atoms
   // A-fragment register sets (8 registers each) in rotation: FRAG_SETS - 1 of the warpgroup's commit groups stay queued
   // while the next is prepared
   static constexpr int FRAG_SETS = BN == 128 ? 4 : 2;
-  // Two CTAs per SM at BN = 64: 128 registers (sm_90a, 0 spills) and 81 KiB of shared memory each.  One at BN = 128:
-  // 223-242 registers, 129 KiB.
+  // Two CTAs per SM at BN = 64: 128 registers (sm_90a, 0 spills) and 81 KiB (image: 97 KiB) of shared memory each.  One at
+  // BN = 128: 223-242 registers, 129 KiB (image: 230 registers, 177 KiB).
   static constexpr int MIN_BLOCKS = BN <= 64 ? 2 : 1;
 };
 
@@ -368,14 +405,17 @@ __device__ __forceinline__ void tile_epilogue(float* stage, const float* s_bias,
   }
 }
 
-// C[m, n] = sum_r A(m, r) * B(n, r) over r in [kbeg, kend) of this split (split z stores at C + z * ep.split_stride).
-template <bool A_KC, bool B_KC, int BN>
-__global__ void __launch_bounds__(NTHREADS, TileCfg<BN>::MIN_BLOCKS)
+// C[m, n] = sum_r A(m, r) * B(n, r) over r in [kbeg, kend) of this split (split z stores at C + z * ep.split_stride).  B_IMG: B is
+// the hi plane of a weight image (row stride ldb = img_ld(K), lo plane img_rows(N) rows behind it), K-major A and B only.
+template <bool A_KC, bool B_KC, int BN, bool B_IMG>
+__global__ void __launch_bounds__(NTHREADS, TileCfg<BN, B_IMG>::MIN_BLOCKS)
 k_gemm_3xtf32(const float* __restrict__ A, int64_t lda, const float* __restrict__ B, int64_t ldb, float* __restrict__ C, int64_t ldc,
               int M, int N, int K, int k_per_split, TcEpilogue ep) {
   static_assert(BN == 64 || BN == 128, "one wgmma.m64nBNk8 per product; two accumulators of BN / 2 registers each");
-  using Cfg = TileCfg<BN>;
+  static_assert(!B_IMG || (A_KC && B_KC), "the image path serves the forward and dgrad GEMMs: K-major A and B");
+  using Cfg = TileCfg<BN, B_IMG>;
   constexpr int NF = Cfg::FRAG_SETS;
+  constexpr int NB = Cfg::B_STAGES, NA = Cfg::A_BUFS;
   static_assert((BK / 8) % NF == 0, "k-step j uses fragment set j % NF in every block");
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(16) float s_bias[BN];
@@ -383,7 +423,7 @@ k_gemm_3xtf32(const float* __restrict__ A, int64_t lda, const float* __restrict_
   uint8_t* smem = smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023);
   auto b_hi = [&](int s) { return smem + s * Cfg::STAGE; };
   auto b_lo = [&](int s) { return b_hi(s) + Cfg::B_BYTES; };
-  float* a_raw = reinterpret_cast<float*>(smem + NSTAGE * Cfg::STAGE);  // two raw A blocks
+  float* a_raw = reinterpret_cast<float*>(smem + NB * Cfg::STAGE);  // NA raw A blocks
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   const int t = lane & 3;
@@ -397,8 +437,9 @@ k_gemm_3xtf32(const float* __restrict__ A, int64_t lda, const float* __restrict_
   pdl_prologue();
   for (int i = threadIdx.x; i < BN; i += NTHREADS) s_bias[i] = (s_bias_on && n0 + i < N) ? ep.bias[n0 + i] : 0.f;
 
-  Loader<B_KC, BN> lb;
-  lb.init(B, ldb, n0, N, kbeg);
+  Loader<B_KC, BN> lb;  // raw B only: unused (and without registers) in the image instantiations
+  if constexpr (!B_IMG) lb.init(B, ldb, n0, N, kbeg);
+  const int64_t plane = B_IMG ? img_rows(N) * ldb : 0;  // image: hi plane -> lo plane
 
   float acc[BN / 2], accx[BN / 2];  // hi*hi chain | cross terms
 #pragma unroll
@@ -407,24 +448,52 @@ k_gemm_3xtf32(const float* __restrict__ A, int64_t lda, const float* __restrict_
 
   if (nkb > 0) {
     a_copy<A_KC>(a_raw, A, lda, m0, M, kbeg, kend - kbeg);
-    lb.load(0, kend - kbeg);
-    lb.store(b_hi(0), b_lo(0));
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor cores
-    cp_async_wait_all();
+    if constexpr (B_IMG) {
+      // commit groups: {A 0, B 0}, {A 1 when two ahead, B 1}; then one group per block (two when A is one ahead, A first), so
+      // that after wait_group 1 only the newest, block kb + 2's B, may still be in flight
+      b_img_copy<BN>(b_hi(0), b_lo(0), B, ldb, plane, n0, kbeg);
+      cp_async_commit();
+      if (nkb > 1) {
+        if (Cfg::A_DIST == 2) a_copy<A_KC>(a_raw + BM * BK, A, lda, m0, M, kbeg + BK, kend - kbeg - BK);
+        b_img_copy<BN>(b_hi(1), b_lo(1), B, ldb, plane, n0, kbeg + BK);
+      }
+      cp_async_commit();
+      cp_async_wait<1>();
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // cp.async writes the generic proxy: -> the tensor cores
+    } else {
+      cp_async_commit();
+      lb.load(0, kend - kbeg);
+      lb.store(b_hi(0), b_lo(0));
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor cores
+      cp_async_wait_all();
+    }
   }
-  int s = 0;  // B stage of block kb
+  int s = 0, sa = 0;  // B stage and (image path) A buffer of block kb; the raw path's A buffer is kb & 1
 #pragma unroll 1
   for (int kb = 0; kb < nkb; ++kb) {
-    // B stage s and A buffer kb & 1 are complete.  Every thread has retired its warpgroup's groups of block kb - 2 (at most
-    // NF - 1 groups are in flight after a wait), so stage (s + 1) % NSTAGE is free for block kb + 1; A buffer (kb + 1) & 1 was
-    // read by block kb - 1's fragment loads.
+    // B stage s and A buffer sa are complete.  Every thread has retired its warpgroup's groups of block kb - 2 (at most NF - 1
+    // groups are in flight after a wait), so B stage (kb - 2) mod NB is free: for block kb + 1 with NB = 3 stages, kb + 2 with
+    // four.  A buffer (kb - 1) mod NA was read by block kb - 1's fragment loads: block kb + NA - 1 goes there.
     __syncthreads();
     const bool more = kb + 1 < nkb;
-    if (more) {  // next block's copies and global loads fly under this block's MMAs
+    if constexpr (B_IMG) {  // copies of block kb + 2 (and of A kb + 1 when it is one ahead) fly under this block's MMAs
+      if (Cfg::A_DIST == 1) {
+        const int k1 = kbeg + (kb + 1) * BK;
+        if (more) a_copy<A_KC>(a_raw + (sa ^ 1) * (BM * BK), A, lda, m0, M, k1, kend - k1);
+        cp_async_commit();
+      }
+      if (kb + 2 < nkb) {
+        const int k2 = kbeg + (kb + 2) * BK, s2 = s + 2 < NB ? s + 2 : s + 2 - NB;
+        if (Cfg::A_DIST == 2) a_copy<A_KC>(a_raw + (sa == 0 ? NA - 1 : sa - 1) * (BM * BK), A, lda, m0, M, k2, kend - k2);
+        b_img_copy<BN>(b_hi(s2), b_lo(s2), B, ldb, plane, n0, k2);
+      }
+      cp_async_commit();  // possibly empty: every block commits the same number of groups
+    } else if (more) {  // next block's copies and global loads fly under this block's MMAs
       a_copy<A_KC>(a_raw + ((kb + 1) & 1) * (BM * BK), A, lda, m0, M, kbeg + (kb + 1) * BK, kend - kbeg - (kb + 1) * BK);
+      cp_async_commit();
       lb.load(kb + 1, kend - kbeg - (kb + 1) * BK);
     }
-    const float* ar = a_raw + (kb & 1) * (BM * BK);
+    const float* ar = a_raw + (B_IMG ? sa : kb & 1) * (BM * BK);
     float4 av[2];  // K-major A: elements 16 (j / 2) + 4t .. + 3 of rows mrow, mrow + 8 (the slots of k-steps j, j + 1 for even j)
     const uint64_t dh = gmma_desc_sw128(smem_u32(b_hi(s))), dl = gmma_desc_sw128(smem_u32(b_lo(s)));
 #pragma unroll
@@ -455,13 +524,20 @@ k_gemm_3xtf32(const float* __restrict__ A, int64_t lda, const float* __restrict_
       wgmma_tf32_rs<BN>(acc, fh[f], dh + 2 * j);
       wgmma_commit();
     }
-    s = s + 1 == NSTAGE ? 0 : s + 1;
+    s = s + 1 == NB ? 0 : s + 1;
+    if constexpr (B_IMG) sa = sa + 1 == NA ? 0 : sa + 1;
     if (more) {
-      lb.store(b_hi(s), b_lo(s));
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      cp_async_wait_all();  // this thread's A copies of block kb + 1 have landed; the barrier publishes them
+      if constexpr (B_IMG) {
+        cp_async_wait<1>();  // this thread's copies of block kb + 1 have landed (block kb + 2's B may still fly)
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      } else {
+        lb.store(b_hi(s), b_lo(s));
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        cp_async_wait_all();  // this thread's A copies of block kb + 1 have landed; the barrier publishes them
+      }
     }
   }
+  if constexpr (B_IMG) cp_async_wait_all();  // only empty groups can be left; nothing may land in the staging tile
   wgmma_wait<0>();
   fence_acc(acc);
   fence_acc(accx);
@@ -505,21 +581,21 @@ k_colsum_tc(const float* __restrict__ gy, int64_t ld, int M, int N, int rows_per
   }
 }
 
-template <bool A_KC, bool B_KC, int BN>
+template <bool A_KC, bool B_KC, int BN, bool B_IMG = false>
 int launch(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N, int K, int splits,
            int k_per_split, const TcEpilogue& ep, cudaStream_t st) {
-  constexpr int smem = TileCfg<BN>::SMEM;
+  constexpr int smem = TileCfg<BN, B_IMG>::SMEM;
   // the shared-memory opt-in belongs to the current device's context: set it once per device (bit d = device d)
   static std::atomic<uint64_t> configured{0};
   int dev = 0;
   PGNN_CUDA(cudaGetDevice(&dev));
   const uint64_t bit = dev < 64 ? (uint64_t)1 << dev : 0;
   if (!(configured.load(std::memory_order_relaxed) & bit)) {
-    PGNN_CUDA(cudaFuncSetAttribute(k_gemm_3xtf32<A_KC, B_KC, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    PGNN_CUDA(cudaFuncSetAttribute(k_gemm_3xtf32<A_KC, B_KC, BN, B_IMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured.fetch_or(bit, std::memory_order_relaxed);
   }
   dim3 grid((unsigned)ceil_div(N, BN), (unsigned)ceil_div(M, BM), (unsigned)splits);
-  PGNN_CUDA(pgnn_launch(k_gemm_3xtf32<A_KC, B_KC, BN>, dim3(grid), dim3(NTHREADS), smem, st, A, lda, B, ldb, C, ldc, M, N, K, k_per_split, ep));
+  PGNN_CUDA(pgnn_launch(k_gemm_3xtf32<A_KC, B_KC, BN, B_IMG>, dim3(grid), dim3(NTHREADS), smem, st, A, lda, B, ldb, C, ldc, M, N, K, k_per_split, ep));
   PGNN_LAUNCH_CHECK();
   return PGNN_OK;
 }
@@ -541,22 +617,114 @@ int dispatch(int bn, const float* A, int64_t lda, const float* B, int64_t ldb, f
   return launch<A_KC, B_KC, 128>(A, lda, B, ldb, C, ldc, M, N, K, splits, k_per_split, ep, st);
 }
 
+// C[M, N] = A[M, K] . B^T from the weight image `img` of B (hi plane first, img_ld(K) floats per row), one split
+int dispatch_img(int bn, const float* A, int64_t lda, const float* img, float* C, int64_t ldc, int M, int N, int K, const TcEpilogue& ep,
+                 cudaStream_t st) {
+  if (ep.hooks.S && (ep.hooks.Q < 1 || ep.hooks.Q > kMaxHookQ)) return PGNN_EINVAL;
+  if (bn == 64) return launch<true, true, 64, true>(A, lda, img, img_ld(K), C, ldc, M, N, K, 1, K, ep, st);
+  return launch<true, true, 128, true>(A, lda, img, img_ld(K), C, ldc, M, N, K, 1, K, ep, st);
+}
+
+// Weight images (see img_rows above) for a batch of weights: job j reads w[rows][cols] (row stride ld) and writes the image of w as
+// a K-major B (B rows = rows, reduction = cols) or, transposed, of w^T (B rows = cols, reduction = rows).  One CTA per 32 x 32 piece
+// of the image; the piece goes through shared memory so that both source orientations are read along their contiguous extent.
+struct PackJob { const float* w; float* img; int64_t ld; int rows, cols, trans; };
+constexpr int kMaxPackJobs = 32;
+struct PackBatch { PackJob job[kMaxPackJobs]; };
+__global__ void __launch_bounds__(256) k_pack_img_batch(PackBatch b) {
+  pdl_prologue();
+  __shared__ float tile[32][33];  // [image row][reduction index]
+  const PackJob j = b.job[blockIdx.z];
+  const int R = j.trans ? j.cols : j.rows, Kr = j.trans ? j.rows : j.cols;
+  const int64_t ld = img_ld(Kr), nr = img_rows(R);
+  const int k0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
+  if (k0 >= ld || r0 >= nr) return;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  for (int i = ty; i < 32; i += 8) {
+    if (j.trans) {  // w^T: image row r0 + tx is column r0 + tx of w
+      const int r = r0 + tx, k = k0 + i;
+      tile[tx][i] = r < R && k < Kr ? j.w[(int64_t)k * j.ld + r] : 0.f;
+    } else {
+      const int r = r0 + i, k = k0 + tx;
+      tile[i][tx] = r < R && k < Kr ? j.w[(int64_t)r * j.ld + k] : 0.f;
+    }
+  }
+  __syncthreads();
+  const int rr = threadIdx.x >> 3, c = (threadIdx.x & 7) * 4;  // one 16-byte piece (slots c .. c + 3) of row r0 + rr per plane
+  float h[4], l[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) split_tf32(tile[rr][kperm(c + q)], h[q], l[q]);
+  float* dst = j.img + (int64_t)(r0 + rr) * ld + k0 + c;
+  *reinterpret_cast<float4*>(dst) = make_float4(h[0], h[1], h[2], h[3]);
+  *reinterpret_cast<float4*>(dst + nr * ld) = make_float4(l[0], l[1], l[2], l[3]);
+}
+
 }  // namespace
 
-extern "C" int pgnn_debug_tc_gemm(int a_kc, int b_kc, int bn, const float* A, int64_t lda, const float* B, int64_t ldb, float* C,
-                                  int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias, int relu, const float* mask,
-                                  int64_t ldm, float* colsum, double* stats, const float* S, int Q, float* gT, float* gT2,
-                                  int q_split, int64_t ldt, void* stream) {
-  PGNN_CHECK_ARG(bn == 64 || bn == 128);
-  PGNN_CHECK_ARG(M > 0 && N > 0 && K > 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31));
-  PGNN_CHECK_ARG(A && B && C && ldc >= N && lda >= (a_kc ? K : M) && ldb >= (b_kc ? K : N));
+// floats of the weight image of a K-major B with `rows` rows and reduction k (both planes)
+int64_t pgnn_tc_image_floats(int64_t rows, int64_t k) { return 2 * img_rows(rows) * img_ld(k); }
+
+// count <= 32 weight images in one launch (PackJob above; rows, cols of the SOURCE w)
+int pgnn_internal_pack_images(int count, const float* const* w, const int64_t* ld, const int* rows, const int* cols, const int* trans,
+                              float* const* img, cudaStream_t st) {
+  if (count <= 0) return PGNN_OK;
+  if (count > kMaxPackJobs) return PGNN_EUNSUPPORTED;
+  PackBatch b;
+  int64_t mr = 0, mk = 0;
+  for (int i = 0; i < count; ++i) {
+    if (!aligned16(img[i])) return PGNN_EUNSUPPORTED;
+    b.job[i] = PackJob{w[i], img[i], ld[i], rows[i], cols[i], trans[i] ? 1 : 0};
+    const int64_t R = img_rows(trans[i] ? cols[i] : rows[i]), K = img_ld(trans[i] ? rows[i] : cols[i]);
+    mr = R > mr ? R : mr;
+    mk = K > mk ? K : mk;
+  }
+  dim3 grid((unsigned)(mk / 32), (unsigned)(mr / 32), (unsigned)count);
+  PGNN_CUDA(pgnn_launch(k_pack_img_batch, dim3(grid), dim3(256), 0, st, b));
+  PGNN_LAUNCH_CHECK();
+  return PGNN_OK;
+}
+
+// The forward and dgrad GEMMs from a weight image (pgnn_internal_pack_images): img_rows / img_k = the image's padded row count and
+// row stride, which must be img_rows(output columns) and img_ld(reduction).  Same epilogues as the raw-weight entry points.
+// y[M,N] = act(x[M,K] . w[N,K]^T + bias), img = the image of w
+int pgnn_tc_linear_fwd_img(const float* x, int64_t ldx, const float* img, int64_t img_r, int64_t img_k, const float* bias, int64_t M,
+                           int64_t N, int64_t K, int relu, float* y, int64_t ldy, cudaStream_t st, const PgnnGemmHooks* hooks) {
+  if (img_r != img_rows(N) || img_k != img_ld(K)) return PGNN_EINVAL;
+  if (ldx % 4 || !aligned16(x) || !aligned16(img) || !aligned16(y) || M < 1) return PGNN_EUNSUPPORTED;
+  TcEpilogue ep{bias, relu, nullptr, 0, 0, hooks ? *hooks : PgnnGemmHooks{}};
+  return dispatch_img(pick_bn((int)M, (int)N, 1), x, ldx, img, y, ldy, (int)M, (int)N, (int)K, ep, st);
+}
+
+// gx[M,K] = (gy[M,N] . w[N,K]) masked by relu_src > 0, img = the image of w^T (B rows K, reduction N)
+int pgnn_tc_linear_bwd_x_img(const float* gy, int64_t ldgy, const float* img, int64_t img_r, int64_t img_k, int64_t M, int64_t N,
+                             int64_t K, const float* relu_src, int64_t ldr, float* gx, int64_t ldgx, cudaStream_t st,
+                             const PgnnGemmHooks* hooks) {
+  if (img_r != img_rows(K) || img_k != img_ld(N)) return PGNN_EINVAL;
+  if (ldgy % 4 || !aligned16(gy) || !aligned16(img) || !aligned16(gx) || M < 1) return PGNN_EUNSUPPORTED;
+  TcEpilogue ep{nullptr, 0, relu_src, ldr, 0, hooks ? *hooks : PgnnGemmHooks{}};
+  return dispatch_img(pick_bn((int)M, (int)K, 1), gy, ldgy, img, gx, ldgx, (int)M, (int)K, (int)N, ep, st);
+}
+
+extern "C" int pgnn_debug_pack_weight_images(int count, const float* const* w, const int64_t* ld, const int32_t* rows,
+                                             const int32_t* cols, const int32_t* transposed, float* const* img, void* stream) {
+  PGNN_CHECK_ARG(count >= 0);
+  if (count == 0) return PGNN_OK;
+  PGNN_CHECK_ARG(w && ld && rows && cols && transposed && img);
+  if (count > kMaxPackJobs) return PGNN_EUNSUPPORTED;
+  for (int i = 0; i < count; ++i) PGNN_CHECK_ARG(w[i] && img[i] && rows[i] > 0 && cols[i] > 0 && ld[i] >= cols[i]);
+  return pgnn_internal_pack_images(count, w, ld, rows, cols, transposed, img, as_stream(stream));
+}
+
+namespace {
+// the epilogue arguments of the two GEMM test entry points
+int debug_epilogue(int64_t N, const float* bias, int relu, const float* mask, int64_t ldm, float* colsum, double* stats, const float* S,
+                   int Q, float* gT, float* gT2, int q_split, int64_t ldt, TcEpilogue& ep) {
   PGNN_CHECK_ARG(!mask || ldm >= N);
   if (S) {
     PGNN_CHECK_ARG(Q >= 1 && Q <= kMaxHookQ && q_split >= 0 && q_split <= Q && ldt >= N);
     PGNN_CHECK_ARG((q_split == 0 || gT) && (q_split == Q || gT2));
   }
-  if (lda % 4 || ldb % 4 || !aligned16(A) || !aligned16(B)) return PGNN_EUNSUPPORTED;
-  TcEpilogue ep{bias, relu, mask, ldm, 0, PgnnGemmHooks{}};
+  ep = TcEpilogue{bias, relu, mask, ldm, 0, PgnnGemmHooks{}};
   ep.hooks.colsum = colsum;
   ep.hooks.stats = stats;
   ep.hooks.S = S;
@@ -565,6 +733,39 @@ extern "C" int pgnn_debug_tc_gemm(int a_kc, int b_kc, int bn, const float* A, in
   ep.hooks.gT2 = gT2;
   ep.hooks.q_split = q_split;
   ep.hooks.ldt = ldt;
+  return PGNN_OK;
+}
+}  // namespace
+
+extern "C" int pgnn_debug_tc_gemm_img(int bn, const float* A, int64_t lda, const float* B, int64_t ldb, float* img, float* C, int64_t ldc,
+                                      int64_t M, int64_t N, int64_t K, const float* bias, int relu, const float* mask, int64_t ldm,
+                                      float* colsum, double* stats, const float* S, int Q, float* gT, float* gT2, int q_split,
+                                      int64_t ldt, void* stream) {
+  PGNN_CHECK_ARG(bn == 64 || bn == 128);
+  PGNN_CHECK_ARG(M > 0 && N > 0 && K > 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31));
+  PGNN_CHECK_ARG(A && B && img && C && ldc >= N && lda >= K && ldb >= K);
+  TcEpilogue ep;
+  const int rc = debug_epilogue(N, bias, relu, mask, ldm, colsum, stats, S, Q, gT, gT2, q_split, ldt, ep);
+  if (rc != PGNN_OK) return rc;
+  if (lda % 4 || ldb % 4 || !aligned16(A) || !aligned16(B) || !aligned16(img)) return PGNN_EUNSUPPORTED;
+  cudaStream_t st = as_stream(stream);
+  const int r = (int)N, c = (int)K, zero = 0;
+  const int prc = pgnn_internal_pack_images(1, &B, &ldb, &r, &c, &zero, &img, st);
+  if (prc != PGNN_OK) return prc;
+  return dispatch_img(bn, A, lda, img, C, ldc, (int)M, (int)N, (int)K, ep, st);
+}
+
+extern "C" int pgnn_debug_tc_gemm(int a_kc, int b_kc, int bn, const float* A, int64_t lda, const float* B, int64_t ldb, float* C,
+                                  int64_t ldc, int64_t M, int64_t N, int64_t K, const float* bias, int relu, const float* mask,
+                                  int64_t ldm, float* colsum, double* stats, const float* S, int Q, float* gT, float* gT2,
+                                  int q_split, int64_t ldt, void* stream) {
+  PGNN_CHECK_ARG(bn == 64 || bn == 128);
+  PGNN_CHECK_ARG(M > 0 && N > 0 && K > 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31));
+  PGNN_CHECK_ARG(A && B && C && ldc >= N && lda >= (a_kc ? K : M) && ldb >= (b_kc ? K : N));
+  TcEpilogue ep;
+  const int rc = debug_epilogue(N, bias, relu, mask, ldm, colsum, stats, S, Q, gT, gT2, q_split, ldt, ep);
+  if (rc != PGNN_OK) return rc;
+  if (lda % 4 || ldb % 4 || !aligned16(A) || !aligned16(B)) return PGNN_EUNSUPPORTED;
   cudaStream_t st = as_stream(stream);
   const int m = (int)M, n = (int)N, k = (int)K;
   if (a_kc && b_kc) return dispatch<true, true>(bn, A, lda, B, ldb, C, ldc, m, n, k, 1, k, ep, st);
@@ -588,15 +789,6 @@ int pgnn_tc_linear_bwd_x(const float* gy, int64_t ldgy, const float* w, int64_t 
   TcEpilogue ep{nullptr, 0, relu_src, ldr, 0, hooks ? *hooks : PgnnGemmHooks{}};
   // output columns are K; the reduction runs over N; B(n_out = k, r = n) = w[r*K + k] is row-index contiguous
   return dispatch<true, false>(pick_bn((int)M, (int)K, 1), gy, ldgy, w, K, gx, ldgx, (int)M, (int)K, (int)N, 1, (int)N, ep, st);
-}
-
-// dgrad with the TRANSPOSED weight at hand: gx[M,K] = gy[M,N] . wT[K,N]^T — both operands reduction-contiguous, so the
-// operand tiles are stored without a transpose (encoder.cu transposes the 2L weight matrices once per backward)
-int pgnn_tc_linear_bwd_x_wt(const float* gy, int64_t ldgy, const float* wT, int64_t M, int64_t N, int64_t K, const float* relu_src,
-                            int64_t ldr, float* gx, int64_t ldgx, cudaStream_t st, const PgnnGemmHooks* hooks) {
-  if (N % 4 || ldgy % 4 || !aligned16(gy) || !aligned16(wT) || !aligned16(gx) || M < 1) return PGNN_EUNSUPPORTED;
-  TcEpilogue ep{nullptr, 0, relu_src, ldr, 0, hooks ? *hooks : PgnnGemmHooks{}};
-  return dispatch<true, true>(pick_bn((int)M, (int)K, 1), gy, ldgy, wT, N, gx, ldgx, (int)M, (int)K, (int)N, 1, (int)N, ep, st);
 }
 
 // out[c][r] = in[r][c] for a batch of row-major matrices (weights: a few hundred KB each)
@@ -729,7 +921,7 @@ int pgnn_tc_linear_bwd_w(const float* gy, int64_t ldgy, const float* x, int64_t 
 }
 
 // test entry points (include/pgnn_b200.h): the weight-gradient GEMM with a caller-chosen split-K workspace, its plan, and the
-// weight-transpose batch of the encoder backward
+// batched transpose
 extern "C" {
 
 int pgnn_debug_tc_wgrad(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,

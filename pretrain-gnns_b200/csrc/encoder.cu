@@ -49,10 +49,14 @@ int pgnn_tc_linear_bwd_w(const float*, int64_t, const float*, int64_t, int64_t, 
 int pgnn_tc_linear_bwd_w_ws(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
                             float* gb, float* partials, int64_t partial_floats, cudaStream_t st);
 int64_t pgnn_tc_wgrad_workspace_floats(int64_t M, int64_t N, int64_t K);
-int pgnn_tc_linear_bwd_x_wt(const float* gy, int64_t ldgy, const float* wT, int64_t M, int64_t N, int64_t K, const float* relu_src,
-                            int64_t ldr, float* gx, int64_t ldgx, cudaStream_t st, const PgnnGemmHooks* hooks);
-int pgnn_internal_transpose_batch(int count, const float* const* in, float* const* out, const int* rows, const int* cols,
-                                  cudaStream_t st);
+int64_t pgnn_tc_image_floats(int64_t rows, int64_t k);
+int pgnn_internal_pack_images(int count, const float* const* w, const int64_t* ld, const int* rows, const int* cols, const int* trans,
+                              float* const* img, cudaStream_t st);
+int pgnn_tc_linear_fwd_img(const float* x, int64_t ldx, const float* img, int64_t img_r, int64_t img_k, const float* bias, int64_t M,
+                           int64_t N, int64_t K, int relu, float* y, int64_t ldy, cudaStream_t st, const PgnnGemmHooks* hooks);
+int pgnn_tc_linear_bwd_x_img(const float* gy, int64_t ldgy, const float* img, int64_t img_r, int64_t img_k, int64_t M, int64_t N,
+                             int64_t K, const float* relu_src, int64_t ldr, float* gx, int64_t ldgx, cudaStream_t st,
+                             const PgnnGemmHooks* hooks);
 int pgnn_internal_bn_apply_fold(const float* x, int64_t ldx, int64_t M, int64_t C, const PgnnBnFold& fold, int relu, float* y,
                                 int64_t ldy, cudaStream_t st, const PgnnDropout* drop);
 int pgnn_internal_bn_fwd_train(const float* x, int64_t ldx, int64_t M, int64_t C, const float* gamma, const float* beta,
@@ -182,7 +186,7 @@ struct GinWs : Front {
   double* bn_acc;                        // [L][2][D] fp64 BatchNorm sums of the forward
   float *aggr, *z1, *z2;                 // [L, N, D], [L, N, 2D], [L, N, D]
   float *gh, *gz2, *gz1, *gaggr;         // backward temporaries
-  float* wT;                             // [L][2][2D*D]: mlp.0.weight^T, mlp.2.weight^T (dgrad B operands)
+  float* wimg;                           // per layer: the weight images of the 2D-row and the D-row B operand (GinImages)
   float* wpart;                          // split-K partial tiles of one wgrad
   int64_t wpart_floats;
   void* scratch;                         // bucket / BatchNorm scratch
@@ -205,7 +209,7 @@ GinWs carve_gin(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
   w.gz2 = c.take<float>(2 * N * D);       // two copies each: layer l's weight-gradient GEMMs (side stream) may still read
   w.gz1 = c.take<float>(2 * N * 2 * D);   // them while layer l-1's backward writes the other copy
   w.gaggr = c.take<float>(N * D);
-  w.wT = c.take<float>(L * 4 * D * D);
+  w.wimg = c.take<float>(L * (pgnn_tc_image_floats(2 * D, D) + pgnn_tc_image_floats(D, 2 * D)));
   w.wpart_floats = split_k_floats(N, 2 * D, D);  // both MLP weight gradients have 2D*D elements
   w.wpart = c.take<float>(w.wpart_floats);
   int64_t sb = pgnn_graph_prep_workspace_bytes(N, E);
@@ -215,6 +219,53 @@ GinWs carve_gin(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
   w.scratch = c.take<char>(sb);
   w.total = c.off;
   return w;
+}
+
+// The weight images of the MLP GEMMs (dense_tc.cu: each weight split into tf32 hi / lo once, in the layout of the GEMM's
+// shared-memory stage).  The forward packs mlp.0.weight and mlp.2.weight as they are, the backward their transposes (the dgrad B
+// operands), into the same workspace region: each pass packs its own, in one launch before its first GEMM.  Per layer the image
+// with 2D rows comes first (mlp.0.weight forward, mlp.2.weight^T backward; reduction D), then the one with D rows (reduction 2D).
+struct GinImages {
+  bool on = false;  // false: the GEMMs read the raw weights (more than 16 layers, precision 0)
+  const float* base = nullptr;
+  int64_t D = 0;
+  static int64_t rows_pad(int64_t rows) { return align_up(rows, 128); }  // the image's padded rows and row stride
+  static int64_t k_pad(int64_t k) { return align_up(k, 32); }
+  const float* wide(int64_t l) const { return base + l * (pgnn_tc_image_floats(2 * D, D) + pgnn_tc_image_floats(D, 2 * D)); }
+  const float* narrow(int64_t l) const { return wide(l) + pgnn_tc_image_floats(2 * D, D); }
+};
+
+int pack_gin_images(const GinWs& w, const void* const* params, int64_t L, int64_t D, bool transposed, cudaStream_t st, GinImages& im) {
+  im = GinImages{};
+  const char* e = getenv("PGNN_WEIGHT_IMAGES");  // =0: the raw-weight GEMMs, for comparing the two paths
+  if (2 * L > 32 || (e && e[0] == '0')) return PGNN_OK;
+  im.base = w.wimg;
+  im.D = D;
+  const float* src[32];
+  float* dst[32];
+  int64_t ld[32];
+  int rows[32], cols[32], tr[32];
+  for (int64_t l = 0; l < L; ++l) {
+    const void* const* p = params + P_LAYER0 + l * L_COUNT;
+    const float* w1 = (const float*)p[L_W1];  // [2D, D]
+    const float* w2 = (const float*)p[L_W2];  // [D, 2D]
+    const int i = (int)(2 * l);
+    src[i] = transposed ? w2 : w1;      // 2D rows
+    src[i + 1] = transposed ? w1 : w2;  // D rows
+    dst[i] = const_cast<float*>(im.wide(l));
+    dst[i + 1] = const_cast<float*>(im.narrow(l));
+    rows[i] = (int)(transposed ? D : 2 * D);
+    cols[i] = (int)(transposed ? 2 * D : D);
+    rows[i + 1] = (int)(transposed ? 2 * D : D);
+    cols[i + 1] = (int)(transposed ? D : 2 * D);
+    ld[i] = cols[i];
+    ld[i + 1] = cols[i + 1];
+    tr[i] = tr[i + 1] = transposed ? 1 : 0;
+  }
+  const int rc = pgnn_internal_pack_images((int)(2 * L), src, ld, rows, cols, tr, dst, st);
+  if (rc == PGNN_OK) im.on = true;
+  else if (rc != PGNN_EUNSUPPORTED) return rc;
+  return PGNN_OK;
 }
 
 struct ConvWs : Front {
@@ -347,6 +398,11 @@ int gin_forward(const void* const* params, void* const* bn_running_mean, void* c
   if (N == 0) return PGNN_OK;
   GinWs w = carve_gin(workspace, N, E, L, D);
   TRY(forward_prologue(kGin, w, params, x, edge_index, edge_attr, N, E, D, training, precision, w.scratch, w.scratch_bytes, stream));
+  cudaStream_t st = as_stream(stream);
+  GinImages im;
+  if (precision == 1) TRY(pack_gin_images(w, params, L, D, false, st, im));
+  const int64_t wide_r = GinImages::rows_pad(2 * D), wide_k = GinImages::k_pad(D);      // mlp.0.weight: 2D rows, reduction D
+  const int64_t narrow_r = GinImages::rows_pad(D), narrow_k = GinImages::k_pad(2 * D);  // mlp.2.weight: D rows, reduction 2D
   const float* h = w.h0;            // input rows of the current layer (pre-affine)
   const float *in_scale = nullptr, *in_shift = nullptr;
   PgnnBnFold fold;                  // pending BatchNorm finalisation of the previous layer (folded into this layer's gather)
@@ -363,7 +419,12 @@ int gin_forward(const void* const* params, void* const* bn_running_mean, void* c
     TRY(pgnn_internal_aggregate_fwd(h, D, in_scale, in_shift, in_scale != nullptr || have_fold, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_SUM,
                                     nullptr, w.S, 9, (const float*)p[L_ET1], (const float*)p[L_ET2], 6, 0, aggr, D, as_stream(stream),
                                     have_fold ? &fold : nullptr, l > 0 ? &drop_in : nullptr));
-    TRY(pgnn_linear_fwd(aggr, D, (const float*)p[L_W1], (const float*)p[L_B1], N, 2 * D, D, 1, z1, 2 * D, precision, stream));
+    int rc1 = im.on ? pgnn_tc_linear_fwd_img(aggr, D, im.wide(l), wide_r, wide_k, (const float*)p[L_B1], N, 2 * D, D, 1, z1, 2 * D, st,
+                                             nullptr)
+                    : PGNN_EUNSUPPORTED;
+    if (rc1 == PGNN_EUNSUPPORTED)
+      rc1 = pgnn_linear_fwd(aggr, D, (const float*)p[L_W1], (const float*)p[L_B1], N, 2 * D, D, 1, z1, 2 * D, precision, stream);
+    if (rc1 != PGNN_OK) return rc1;
     have_fold = false;
     // GEMM2; on the tensor path its epilogue also accumulates the BatchNorm batch statistics of z2 (fp64 atomics)
     bool stats_fused = false;
@@ -372,12 +433,22 @@ int gin_forward(const void* const* params, void* const* bn_running_mean, void* c
       PGNN_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * 2 * D, as_stream(stream)));
       PgnnGemmHooks hk;
       hk.stats = acc;
-      const int rc = pgnn_tc_linear_fwd(z1, 2 * D, (const float*)p[L_W2], (const float*)p[L_B2], N, D, 2 * D, 0, z2, D, as_stream(stream), &hk);
+      int rc = im.on ? pgnn_tc_linear_fwd_img(z1, 2 * D, im.narrow(l), narrow_r, narrow_k, (const float*)p[L_B2], N, D, 2 * D, 0, z2, D,
+                                              st, &hk)
+                     : PGNN_EUNSUPPORTED;
+      if (rc == PGNN_EUNSUPPORTED)
+        rc = pgnn_tc_linear_fwd(z1, 2 * D, (const float*)p[L_W2], (const float*)p[L_B2], N, D, 2 * D, 0, z2, D, st, &hk);
       if (rc == PGNN_OK) stats_fused = true;
       else if (rc != PGNN_EUNSUPPORTED) return rc;
     }
-    if (!stats_fused)
-      TRY(pgnn_linear_fwd(z1, 2 * D, (const float*)p[L_W2], (const float*)p[L_B2], N, D, 2 * D, 0, z2, D, precision, stream));
+    if (!stats_fused) {
+      int rc = im.on && !training ? pgnn_tc_linear_fwd_img(z1, 2 * D, im.narrow(l), narrow_r, narrow_k, (const float*)p[L_B2], N, D,
+                                                           2 * D, 0, z2, D, st, nullptr)
+                                  : PGNN_EUNSUPPORTED;
+      if (rc == PGNN_EUNSUPPORTED)
+        rc = pgnn_linear_fwd(z1, 2 * D, (const float*)p[L_W2], (const float*)p[L_B2], N, D, 2 * D, 0, z2, D, precision, stream);
+      if (rc != PGNN_OK) return rc;
+    }
     if (training && stats_fused) {
       // no finalize launch: the consumer (next layer's gather, or the final apply) derives scale/shift from the sums
       fold = PgnnBnFold{};
@@ -429,22 +500,11 @@ int gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg
   }
   PGNN_CHECK_ARG(g_node_rep && x);
   GinWs w = carve_gin(workspace, N, E, L, D);
-  // transposed copies of the 2L MLP weights: with them every dgrad has both operands reduction-contiguous, and the GEMM
-  // stores its operand tiles without a transpose
-  bool have_wT = false;
-  if (precision == 1 && 2 * L <= 32) {
-    const float* in[32];
-    float* out[32];
-    int rows[32], cols[32];
-    for (int64_t l = 0; l < L; ++l) {
-      const void* const* p = params + P_LAYER0 + l * L_COUNT;
-      in[2 * l] = (const float*)p[L_W1];     out[2 * l] = w.wT + (2 * l) * 2 * D * D;     rows[2 * l] = (int)(2 * D); cols[2 * l] = (int)D;
-      in[2 * l + 1] = (const float*)p[L_W2]; out[2 * l + 1] = w.wT + (2 * l + 1) * 2 * D * D; rows[2 * l + 1] = (int)D; cols[2 * l + 1] = (int)(2 * D);
-    }
-    const int rc = pgnn_internal_transpose_batch((int)(2 * L), in, out, rows, cols, st);
-    if (rc == PGNN_OK) have_wT = true;
-    else if (rc != PGNN_EUNSUPPORTED) return rc;
-  }
+  // images of the transposed MLP weights: the dgrad B operands, reduction-contiguous and already split
+  GinImages im;
+  if (precision == 1) TRY(pack_gin_images(w, params, L, D, true, st, im));
+  const int64_t wide_r = GinImages::rows_pad(2 * D), wide_k = GinImages::k_pad(D);      // mlp.2.weight^T: 2D rows, reduction D
+  const int64_t narrow_r = GinImages::rows_pad(D), narrow_k = GinImages::k_pad(2 * D);  // mlp.0.weight^T: D rows, reduction 2D
   const float* gy = g_node_rep;
   int64_t ldgy = ldg;
   SideCtx* sc = precision == 1 ? side_ctx(st) : nullptr;
@@ -483,8 +543,8 @@ int gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg
         PGNN_CUDA(cudaMemsetAsync(grads + o[L_B1], 0, sizeof(float) * 2 * D, st));
         PgnnGemmHooks h1;
         h1.colsum = grads + o[L_B1];
-        rc = have_wT ? pgnn_tc_linear_bwd_x_wt(gz2, D, w.wT + (2 * l + 1) * 2 * D * D, N, D, 2 * D, z1, 2 * D, gz1, 2 * D, st, &h1)
-                     : PGNN_EUNSUPPORTED;
+        rc = im.on ? pgnn_tc_linear_bwd_x_img(gz2, D, im.wide(l), wide_r, wide_k, N, D, 2 * D, z1, 2 * D, gz1, 2 * D, st, &h1)
+                   : PGNN_EUNSUPPORTED;
         if (rc == PGNN_EUNSUPPORTED)
           rc = pgnn_tc_linear_bwd_x(gz2, D, (const float*)p[L_W2], N, D, 2 * D, z1, 2 * D, gz1, 2 * D, st, &h1);
         if (rc != PGNN_OK) return rc;
@@ -498,8 +558,8 @@ int gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg
         PGNN_CUDA(cudaMemsetAsync(grads + o[L_ET1], 0, sizeof(float) * 9 * D, st));  // the two tables are adjacent in the layout
         PgnnGemmHooks h2;
         h2.S = w.S; h2.Q = 9; h2.gT = grads + o[L_ET1]; h2.gT2 = grads + o[L_ET2]; h2.q_split = 6; h2.ldt = D;
-        rc = have_wT ? pgnn_tc_linear_bwd_x_wt(gz1, 2 * D, w.wT + (2 * l) * 2 * D * D, N, 2 * D, D, nullptr, 0, w.gaggr, D, st, &h2)
-                     : PGNN_EUNSUPPORTED;
+        rc = im.on ? pgnn_tc_linear_bwd_x_img(gz1, 2 * D, im.narrow(l), narrow_r, narrow_k, N, 2 * D, D, nullptr, 0, w.gaggr, D, st, &h2)
+                   : PGNN_EUNSUPPORTED;
         if (rc == PGNN_EUNSUPPORTED)
           rc = pgnn_tc_linear_bwd_x(gz1, 2 * D, (const float*)p[L_W1], N, 2 * D, D, nullptr, 0, w.gaggr, D, st, &h2);
         if (rc != PGNN_OK) return rc;

@@ -1,6 +1,7 @@
 """Per-shape timing of the 3xTF32 wgmma GEMM (k_gemm_3xtf32): the six GEMMs of one GIN-300 layer as csrc/encoder.cu issues them
 on the masking step, at that batch's node count N, each through the library's test entry points with the same tile width,
-epilogue hooks and split-K workspace the encoder gets.  Prints one JSON line per (library, GEMM): us per call, TFLOP/s
+epilogue hooks and split-K workspace the encoder gets.  The four with a weight as B (fwd1, fwd2, dgrad2, dgrad1) run twice: from
+the raw weight, and from the weight image the encoder packs once per pass ("img" lines: GEMM only, the pack is not timed).  Prints one JSON line per (library, GEMM): us per call, TFLOP/s
 (2 N K_in K_out over the time) and the fraction of 165 TFLOP/s, the 3xTF32 ceiling of a 495 TFLOP/s dense-TF32 H100 SXM.
 
     python tools/bench_gemm.py [--rows 5930] [--reps 200] [--rounds 1] [--lib PATH ...]
@@ -57,11 +58,16 @@ def child(rows, reps, label):
         assert lib.pgnn_debug_tc_wgrad_plan(M, Nn, K, out) == 0
         return list(out)
 
+    img = torch.empty(2 * 640 * 320 + 2 * 384 * 608, device=dev)  # room for either image shape of the layer
+
     part2, part1 = (torch.empty(plan(N, n, k)[2] * n * k, device=dev) for n, k in ((D, 2 * D), (2 * D, D)))
     p = lambda t: t.data_ptr()
 
-    def gemm(A, B, C, K, Nout, bias=None, relu=0, mask=None, colsum=None, stats=None, S=None):
-        rc = lib.pgnn_debug_tc_gemm(1, 1, pick_bn(N, Nout), p(A), A.shape[1], p(B), B.shape[1], p(C), C.shape[1], N, Nout, K,
+    def gemm(A, B, C, K, Nout, bias=None, relu=0, mask=None, colsum=None, stats=None, S=None, image=False):
+        # image: pgnn_debug_tc_gemm_img, which packs B into the image and runs the GEMM from it (the "pack" lines time the pack alone)
+        head = (pick_bn(N, Nout), p(A), A.shape[1], p(B), B.shape[1], p(img)) if image else (1, 1, pick_bn(N, Nout), p(A), A.shape[1],
+                                                                                          p(B), B.shape[1])
+        rc = (lib.pgnn_debug_tc_gemm_img if image else lib.pgnn_debug_tc_gemm)(*head, p(C), C.shape[1], N, Nout, K,
                                     p(bias) if bias is not None else None, relu, p(mask) if mask is not None else None,
                                     mask.shape[1] if mask is not None else 0, p(colsum) if colsum is not None else None,
                                     p(stats) if stats is not None else None, p(S) if S is not None else None, 9 if S is not None else 0,
@@ -74,6 +80,13 @@ def child(rows, reps, label):
                                      part.numel(), st)
         assert rc == 0, rc
 
+    def pack(B):
+        one = lambda t, c: (c * 1)(t)
+        rc = lib.pgnn_debug_pack_weight_images(1, one(p(B), ctypes.c_void_p), one(B.shape[1], ctypes.c_int64),
+                                               one(B.shape[0], ctypes.c_int32), one(B.shape[1], ctypes.c_int32), one(0, ctypes.c_int32),
+                                               one(p(img), ctypes.c_void_p), st)
+        assert rc == 0, rc
+
     cases = [  # (name, output columns, reduction, tile width, splits, call)
         ("fwd1 300->600 +bias ReLU", 2 * D, D, pick_bn(N, 2 * D), 1, lambda: gemm(aggr, w1, y1, D, 2 * D, bias=b1, relu=1)),
         ("fwd2 600->300 +bias stats", D, 2 * D, pick_bn(N, D), 1, lambda: gemm(z1, w2, y2, 2 * D, D, bias=b2, stats=stats)),
@@ -82,6 +95,14 @@ def child(rows, reps, label):
         ("dgrad1 600->300 S-hook", D, 2 * D, pick_bn(N, D), 1, lambda: gemm(gz1, w1T, gx0, 2 * D, D, S=S)),
         ("wgrad2 [300,600] split-K", D, 2 * D, *plan(N, D, 2 * D)[0:3:2], lambda: wgrad(gz2, z1, gw2, part2)),
         ("wgrad1 [600,300] split-K", 2 * D, D, *plan(N, 2 * D, D)[0:3:2], lambda: wgrad(gz1, aggr, gw1, part1)),
+    ]
+    cases += [
+        ("fwd1 img (+pack)", 2 * D, D, pick_bn(N, 2 * D), 1, lambda: gemm(aggr, w1, y1, D, 2 * D, bias=b1, relu=1, image=True)),
+        ("fwd2 img (+pack)", D, 2 * D, pick_bn(N, D), 1, lambda: gemm(z1, w2, y2, 2 * D, D, bias=b2, stats=stats, image=True)),
+        ("dgrad2 img (+pack)", 2 * D, D, pick_bn(N, 2 * D), 1, lambda: gemm(gz2, w2T, gx1, D, 2 * D, mask=z1, colsum=colsum, image=True)),
+        ("dgrad1 img (+pack)", D, 2 * D, pick_bn(N, D), 1, lambda: gemm(gz1, w1T, gx0, 2 * D, D, S=S, image=True)),
+        ("pack [600,300]", 0, 0, 0, 1, lambda: pack(w1)),
+        ("pack [300,600]", 0, 0, 0, 1, lambda: pack(w2)),
     ]
     name = torch.cuda.get_device_name(0)
     for title, n_out, k, bn, splits, fn in cases:
