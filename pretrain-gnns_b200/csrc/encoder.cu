@@ -23,8 +23,10 @@
 // library-defined layout of pgnn_chem_gin_grad_offsets / pgnn_chem_conv_grad_offsets (grad_layout below), which is also the
 // buffer the data-parallel all-reduce runs on.
 //
-// The bio GNN (bio/model.py, pgnn_bio_encoder_*) has its own layer bodies at the end of the file on the same scaffolding:
-// workspace carving (Carve / Front), Drops, the side-stream weight gradients (SideCtx) and a flat gradient layout.
+// The bio GNN (bio/model.py, pgnn_bio_encoder_*) runs on the same scaffolding: workspace carving (Carve / Front / Tail), Drops,
+// the side-stream weight gradients (side_wgrad) and a flat gradient layout.  Its GIN has a layer body of its own (bio_gin_*);
+// GCN / GraphSAGE / GAT share one body with chem (conv_forward / conv_backward), the domain filling in the layer's edge term
+// (EdgeTerm) and the step around the conv: chem's BatchNorm, bio's ReLU + dropout sweep.
 #include "common.cuh"
 
 #include <cstdlib>
@@ -45,7 +47,6 @@ int pgnn_tc_linear_fwd(const float*, int64_t, const float*, const float*, int64_
                        cudaStream_t, const PgnnGemmHooks*);
 int pgnn_tc_linear_bwd_x(const float*, int64_t, const float*, int64_t, int64_t, int64_t, const float*, int64_t, float*, int64_t,
                          cudaStream_t, const PgnnGemmHooks*);
-int pgnn_tc_linear_bwd_w(const float*, int64_t, const float*, int64_t, int64_t, int64_t, int64_t, float*, float*, cudaStream_t);
 int pgnn_tc_linear_bwd_w_ws(const float* gy, int64_t ldgy, const float* x, int64_t ldx, int64_t M, int64_t N, int64_t K, float* gw,
                             float* gb, float* partials, int64_t partial_floats, cudaStream_t st);
 int64_t pgnn_tc_wgrad_workspace_floats(int64_t M, int64_t N, int64_t K);
@@ -75,6 +76,8 @@ constexpr int kAtomRows = 120, kChiralRows = 3;   // chem/model.py:9-10
 constexpr int kOneHotLd = 124;                    // kAtomRows + kChiralRows padded to a multiple of 4
 constexpr int kHeads = 2;          // chem/model.py:108 (heads=2 is what GNN.__init__ builds, :243)
 constexpr float kSlope = 0.2f;     // negative_slope, chem/model.py:108
+constexpr int kChemQ = 9, kChemQSplit = 6;  // chem S columns: 6 bond-type rows (edge_embedding1), then 3 direction rows
+constexpr int kBioQ = 10;          // bio S columns: the 9 edge attributes + the weight sum that multiplies the encoder bias
 
 // order of the parameter pointer table and of the flat gradient layout
 enum { P_XEMB1 = 0, P_XEMB2 = 1, P_LAYER0 = 2 };
@@ -82,10 +85,14 @@ enum { P_XEMB1 = 0, P_XEMB2 = 1, P_LAYER0 = 2 };
 enum { L_W1 = 0, L_B1, L_W2, L_B2, L_ET1, L_ET2, L_GAMMA, L_BETA, L_COUNT };     // gin
 enum { G_W = 0, G_B, G_ET1, G_ET2, G_GAMMA, G_BETA, G_COUNT };                    // gcn / graphsage
 enum { A_W = 0, A_B, A_ATT, A_BIAS, A_ET1, A_ET2, A_GAMMA, A_BETA, A_COUNT };     // gat
+// the leading parameters of a conv layer, the same in both domains (BioParam below): the Linear, then GAT's att and bias
+constexpr int CV_W = 0, CV_B = 1, CV_ATT = 2, CV_BIAS = 3;
+static_assert(G_W == CV_W && G_B == CV_B && A_W == CV_W && A_B == CV_B && A_ATT == CV_ATT && A_BIAS == CV_BIAS, "chem conv order");
 
 inline int layer_params(int type) { return type == kGin ? L_COUNT : type == PGNN_CONV_GAT ? A_COUNT : G_COUNT; }
 inline int agg_mode(int type) { return type == kGin ? PGNN_AGG_SUM : type == PGNN_CONV_GCN ? PGNN_AGG_GCN : PGNN_AGG_MEAN; }
 bool valid_conv(int t) { return t == PGNN_CONV_GCN || t == PGNN_CONV_SAGE || t == PGNN_CONV_GAT; }
+bool valid_type(int t) { return t == kGin || valid_conv(t); }
 
 // Per-layer dropout of one pass: layer l's mask is PgnnDropout(p, seed, l).  p == 0 (or eval mode) leaves every layer without
 // one, so the kernels without a mask run.
@@ -97,6 +104,17 @@ struct Drops {
     pgnn_make_dropout(p, seed, l, &d);
     return d;
   }
+};
+
+// The BatchNorm running state of a pass (one pointer per layer; nbt may be null) and its hyper-parameters
+struct BnRun {
+  void* const* mean = nullptr;
+  void* const* var = nullptr;
+  void* const* nbt = nullptr;
+  float momentum = 0.f, eps = 0.f;
+  float* rm(int64_t l) const { return (float*)mean[l]; }
+  float* rv(int64_t l) const { return (float*)var[l]; }
+  int64_t* nb(int64_t l) const { return nbt ? (int64_t*)nbt[l] : nullptr; }
 };
 
 #define TRY(call)                     \
@@ -136,30 +154,27 @@ int64_t grad_layout(int type, int64_t L, int64_t D, int64_t* offsets) {
   return i;
 }
 
-// 256-byte aligned regions of one workspace (base == nullptr only measures).  With `pad_empty` an empty region still takes one
-// element, as every conv region does; GIN's regions take no space when empty, except its edge arrays (carve_front).
+// 256-byte aligned regions of one workspace (base == nullptr only measures); an empty region takes no space
 struct Carve {
   char* base;
-  bool pad_empty;
   int64_t off = 0;
-  Carve(void* b, bool pad) : base(reinterpret_cast<char*>(b)), pad_empty(pad) {}
+  explicit Carve(void* b) : base(reinterpret_cast<char*>(b)) {}
   template <typename T>
   T* take(int64_t count) {
     T* p = reinterpret_cast<T*>(base + off);
-    off += align_up((pad_empty && count < 1 ? 1 : count) * (int64_t)sizeof(T), 256);
+    off += align_up(count * (int64_t)sizeof(T), 256);
     return p;
   }
 };
 
-// the first regions of every type's workspace: what forward_prologue writes
+// the first regions of every workspace: what the prologues write
 struct Front {
   int32_t *rowptr_t, *rowptr_s, *nbr_t, *eid_t, *nbr_s, *eid_s;
   float *S, *dinv, *h0;  // dinv: conv types only
-  float* onehot;         // [N, kOneHotLd]: atom-code one-hot rows (embedding gradient as a GEMM)
+  float* onehot;         // chem: [N, kOneHotLd] atom-code one-hot rows (embedding gradient as a GEMM)
 };
 
-// Q: the summary's columns (9 chem, 10 bio); onehot_ld: the one-hot rows' width (0: none, bio)
-void carve_front(Carve& c, Front& f, int type, int64_t N, int64_t E, int64_t D, int64_t Q = 9, int64_t onehot_ld = kOneHotLd) {
+void carve_front(Carve& c, Front& f, bool bio, int type, int64_t N, int64_t E, int64_t D) {
   const int64_t e1 = E > 0 ? E : 1;
   f.rowptr_t = c.take<int32_t>(N + 1);
   f.rowptr_s = c.take<int32_t>(N + 1);
@@ -167,36 +182,59 @@ void carve_front(Carve& c, Front& f, int type, int64_t N, int64_t E, int64_t D, 
   f.eid_t = c.take<int32_t>(e1);
   f.nbr_s = c.take<int32_t>(e1);
   f.eid_s = c.take<int32_t>(e1);
-  f.S = c.take<float>(N * Q);
+  f.S = c.take<float>(N * (bio ? kBioQ : kChemQ));
   f.dinv = type == kGin ? nullptr : c.take<float>(N);
   f.h0 = c.take<float>(N * D);
-  f.onehot = onehot_ld ? c.take<float>(N * onehot_ld) : nullptr;
+  f.onehot = bio ? nullptr : c.take<float>(N * kOneHotLd);
 }
 
-// split-K partial tiles for the largest weight-gradient GEMM of a type: its layer wgrads ([N_out, D] with N_out = the given
-// width) and the embedding tables' gradient as a GEMM
+// the last regions of every workspace: split-K partial tiles of the largest weight-gradient GEMM, and one scratch shared by graph
+// preparation, the BatchNorms (bn_width: the widest one; 0: none) and the GAT backward
+struct Tail {
+  float* wpart;
+  int64_t wpart_floats;
+  void* scratch;
+  int64_t scratch_bytes, total;
+};
+
+void carve_tail(Carve& c, Tail& t, int type, int64_t N, int64_t E, int64_t D, int64_t wpart_floats, int64_t bn_width) {
+  t.wpart_floats = wpart_floats;
+  t.wpart = c.take<float>(wpart_floats);
+  int64_t sb = pgnn_graph_prep_workspace_bytes(N, E);
+  const int64_t bb = bn_width ? pgnn_bn_workspace_bytes(N > 0 ? N : 1, bn_width) : 0;
+  const int64_t gb = type == PGNN_CONV_GAT ? pgnn_gat_bwd_workspace_bytes(N, E, kHeads, D) : 0;
+  if (bb > sb) sb = bb;
+  if (gb > sb) sb = gb;
+  t.scratch_bytes = sb;
+  t.scratch = c.take<char>(sb);
+  t.total = c.off;
+}
+
+// chem split-K partial tiles: the layer wgrads ([width, D] over N rows) and the embedding tables' gradient as a GEMM
 int64_t split_k_floats(int64_t N, int64_t width, int64_t D) {
   const int64_t a = pgnn_tc_wgrad_workspace_floats(N, width, D);
   const int64_t e = pgnn_tc_wgrad_workspace_floats(N, kAtomRows + kChiralRows, D);
   return e > a ? e : a;
 }
 
-struct GinWs : Front {
+struct GinWs : Front, Tail {
   float *scale, *shift, *mean, *invstd;  // [L, D]
   double* bn_acc;                        // [L][2][D] fp64 BatchNorm sums of the forward
   float *aggr, *z1, *z2;                 // [L, N, D], [L, N, 2D], [L, N, D]
   float *gh, *gz2, *gz1, *gaggr;         // backward temporaries
   float* wimg;                           // per layer: the weight images of the 2D-row and the D-row B operand (GinImages)
-  float* wpart;                          // split-K partial tiles of one wgrad
-  int64_t wpart_floats;
-  void* scratch;                         // bucket / BatchNorm scratch
-  int64_t scratch_bytes, total;
 };
 
+// The weight images of the MLP GEMMs (dense_tc.cu: each weight split into tf32 hi / lo once, in the layout of the GEMM's
+// shared-memory stage).  The forward packs mlp.0.weight and mlp.2.weight as they are, the backward their transposes (the dgrad B
+// operands), into the same workspace region: each pass packs its own, in one launch before its first GEMM.  Per layer the image
+// with 2D rows comes first (mlp.0.weight forward, mlp.2.weight^T backward; reduction D), then the one with D rows (reduction 2D).
+inline int64_t gin_image_floats(int64_t D) { return pgnn_tc_image_floats(2 * D, D) + pgnn_tc_image_floats(D, 2 * D); }
+
 GinWs carve_gin(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
-  Carve c(base, false);
+  Carve c(base);
   GinWs w;
-  carve_front(c, w, kGin, N, E, D);
+  carve_front(c, w, false, kGin, N, E, D);
   w.bn_acc = c.take<double>(L * 2 * D);
   w.scale = c.take<float>(L * D);
   w.shift = c.take<float>(L * D);
@@ -209,38 +247,63 @@ GinWs carve_gin(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
   w.gz2 = c.take<float>(2 * N * D);       // two copies each: layer l's weight-gradient GEMMs (side stream) may still read
   w.gz1 = c.take<float>(2 * N * 2 * D);   // them while layer l-1's backward writes the other copy
   w.gaggr = c.take<float>(N * D);
-  w.wimg = c.take<float>(L * (pgnn_tc_image_floats(2 * D, D) + pgnn_tc_image_floats(D, 2 * D)));
-  w.wpart_floats = split_k_floats(N, 2 * D, D);  // both MLP weight gradients have 2D*D elements
-  w.wpart = c.take<float>(w.wpart_floats);
-  int64_t sb = pgnn_graph_prep_workspace_bytes(N, E);
-  const int64_t bb = pgnn_bn_workspace_bytes(N > 0 ? N : 1, D);
-  if (bb > sb) sb = bb;
-  w.scratch_bytes = sb;
-  w.scratch = c.take<char>(sb);
-  w.total = c.off;
+  w.wimg = c.take<float>(L * gin_image_floats(D));
+  carve_tail(c, w, kGin, N, E, D, split_k_floats(N, 2 * D, D), D);  // both MLP weight gradients have 2D*D elements
   return w;
 }
 
-// The weight images of the MLP GEMMs (dense_tc.cu: each weight split into tf32 hi / lo once, in the layout of the GEMM's
-// shared-memory stage).  The forward packs mlp.0.weight and mlp.2.weight as they are, the backward their transposes (the dgrad B
-// operands), into the same workspace region: each pass packs its own, in one launch before its first GEMM.  Per layer the image
-// with 2D rows comes first (mlp.0.weight forward, mlp.2.weight^T backward; reduction D), then the one with D rows (reduction 2D).
+// GCN / GraphSAGE / GAT of both domains; C = the Linear's width (H*D for GAT), Q = the summary's columns
+struct ConvWs : Front, Tail {
+  float *T, *xl, *z, *hout;    // [L][Q][C] tables (bio; chem GAT); per layer: Linear output [N, C], conv output [N, D], layer output [N, D]
+  float *nrm, *alpha, *pq;     // per layer: SAGE row norms [N]; GAT attention [(E+N), H] and logit halves [N, H, 2]
+  float *mean, *invstd;        // chem: BatchNorm batch statistics [L, D]
+  float *gz, *ga, *gxl, *gh;   // backward temporaries [N, D], [N, D], two copies of [N, C] by layer parity, [N, D]
+  float* gT;                   // bio: table gradients [L][Q][C]
+};
+
+ConvWs carve_conv(void* base, bool bio, int type, int64_t N, int64_t E, int64_t L, int64_t D) {
+  Carve c(base);
+  ConvWs w;
+  const bool gat = type == PGNN_CONV_GAT;
+  const int64_t C = gat ? kHeads * D : D, Q = bio ? kBioQ : kChemQ;
+  carve_front(c, w, bio, type, N, E, D);
+  w.T = c.take<float>(bio || gat ? L * Q * C : 0);
+  w.xl = c.take<float>(L * N * C);
+  w.z = c.take<float>(L * N * D);
+  w.hout = c.take<float>(L * N * D);
+  w.nrm = c.take<float>(type == PGNN_CONV_SAGE ? L * N : 0);
+  w.alpha = c.take<float>(gat ? L * (E + N) * kHeads : 0);
+  w.pq = c.take<float>(gat ? L * N * kHeads * 2 : 0);
+  w.mean = c.take<float>(bio ? 0 : L * D);
+  w.invstd = c.take<float>(bio ? 0 : L * D);
+  w.gz = c.take<float>(N * D);
+  w.ga = c.take<float>(N * D);
+  w.gxl = c.take<float>(2 * N * C);   // two copies by layer parity: the side-stream wgrad of layer l reads one while layer l-1 writes the other
+  w.gh = c.take<float>(N * D);
+  w.gT = c.take<float>(bio ? L * Q * C : 0);
+  carve_tail(c, w, type, N, E, D, bio ? pgnn_tc_wgrad_workspace_floats(N, C, D) : split_k_floats(N, C, D), bio ? 0 : D);
+  return w;
+}
+
+// A tensor-path GEMM's weight operand as an image: its base, padded row count and row stride.  w == nullptr: no image.
+struct Img {
+  const float* w = nullptr;
+  int64_t rows = 0, k = 0;
+};
+
 struct GinImages {
-  bool on = false;  // false: the GEMMs read the raw weights (more than 16 layers, precision 0)
-  const float* base = nullptr;
+  const float* base = nullptr;  // nullptr: the GEMMs read the raw weights (more than 16 layers, precision 0)
   int64_t D = 0;
-  static int64_t rows_pad(int64_t rows) { return align_up(rows, 128); }  // the image's padded rows and row stride
-  static int64_t k_pad(int64_t k) { return align_up(k, 32); }
-  const float* wide(int64_t l) const { return base + l * (pgnn_tc_image_floats(2 * D, D) + pgnn_tc_image_floats(D, 2 * D)); }
-  const float* narrow(int64_t l) const { return wide(l) + pgnn_tc_image_floats(2 * D, D); }
+  Img wide(int64_t l) const { return base ? Img{base + l * gin_image_floats(D), align_up(2 * D, 128), align_up(D, 32)} : Img{}; }
+  Img narrow(int64_t l) const {
+    return base ? Img{base + l * gin_image_floats(D) + pgnn_tc_image_floats(2 * D, D), align_up(D, 128), align_up(2 * D, 32)} : Img{};
+  }
 };
 
 int pack_gin_images(const GinWs& w, const void* const* params, int64_t L, int64_t D, bool transposed, cudaStream_t st, GinImages& im) {
   im = GinImages{};
   const char* e = getenv("PGNN_WEIGHT_IMAGES");  // =0: the raw-weight GEMMs, for comparing the two paths
   if (2 * L > 32 || (e && e[0] == '0')) return PGNN_OK;
-  im.base = w.wimg;
-  im.D = D;
   const float* src[32];
   float* dst[32];
   int64_t ld[32];
@@ -252,8 +315,8 @@ int pack_gin_images(const GinWs& w, const void* const* params, int64_t L, int64_
     const int i = (int)(2 * l);
     src[i] = transposed ? w2 : w1;      // 2D rows
     src[i + 1] = transposed ? w1 : w2;  // D rows
-    dst[i] = const_cast<float*>(im.wide(l));
-    dst[i + 1] = const_cast<float*>(im.narrow(l));
+    dst[i] = w.wimg + l * gin_image_floats(D);
+    dst[i + 1] = dst[i] + pgnn_tc_image_floats(2 * D, D);
     rows[i] = (int)(transposed ? D : 2 * D);
     cols[i] = (int)(transposed ? 2 * D : D);
     rows[i + 1] = (int)(transposed ? 2 * D : D);
@@ -263,62 +326,69 @@ int pack_gin_images(const GinWs& w, const void* const* params, int64_t L, int64_
     tr[i] = tr[i + 1] = transposed ? 1 : 0;
   }
   const int rc = pgnn_internal_pack_images((int)(2 * L), src, ld, rows, cols, tr, dst, st);
-  if (rc == PGNN_OK) im.on = true;
+  if (rc == PGNN_OK) im = GinImages{w.wimg, D};
   else if (rc != PGNN_EUNSUPPORTED) return rc;
   return PGNN_OK;
 }
 
-struct ConvWs : Front {
-  float *xl, *z, *hout;        // per layer: Linear output [N, HD], BatchNorm input [N, D], layer output [N, D]
-  float *nrm, *alpha, *pq, *T; // per layer: SAGE row norms [N]; GAT attention [(E+N), H], logit halves [N, H, 2], tables [9, HD]
-  float *mean, *invstd;        // [L, D]
-  float *gz, *ga, *gxl, *gh;   // backward temporaries [N, D], [N, D], [N, HD], [N, D]
-  float* wpart;
-  int64_t wpart_floats;
-  void* scratch;
-  int64_t scratch_bytes, total;
-};
-
-ConvWs carve_conv(void* base, int type, int64_t N, int64_t E, int64_t L, int64_t D) {
-  Carve c(base, true);
-  ConvWs w;
-  const int64_t HD = type == PGNN_CONV_GAT ? kHeads * D : D;
-  carve_front(c, w, type, N, E, D);
-  w.xl = c.take<float>(L * N * HD);
-  w.z = c.take<float>(L * N * D);
-  w.hout = c.take<float>(L * N * D);
-  w.nrm = c.take<float>(type == PGNN_CONV_SAGE ? L * N : 0);
-  w.alpha = c.take<float>(type == PGNN_CONV_GAT ? L * (E + N) * kHeads : 0);
-  w.pq = c.take<float>(type == PGNN_CONV_GAT ? L * N * kHeads * 2 : 0);
-  w.T = c.take<float>(type == PGNN_CONV_GAT ? L * 9 * HD : 0);
-  w.mean = c.take<float>(L * D);
-  w.invstd = c.take<float>(L * D);
-  w.gz = c.take<float>(N * D);
-  w.ga = c.take<float>(N * D);
-  w.gxl = c.take<float>(2 * N * HD);   // two copies by layer parity: the side-stream wgrad of layer l reads one while layer l-1 writes the other
-  w.gh = c.take<float>(N * D);
-  w.wpart_floats = split_k_floats(N, HD, D);
-  w.wpart = c.take<float>(w.wpart_floats);
-  int64_t sb = pgnn_graph_prep_workspace_bytes(N, E);
-  const int64_t bb = pgnn_bn_workspace_bytes(N > 0 ? N : 1, D);
-  if (bb > sb) sb = bb;
-  if (type == PGNN_CONV_GAT) {
-    const int64_t gb = pgnn_gat_bwd_workspace_bytes(N, E, kHeads, D);
-    if (gb > sb) sb = gb;
-  }
-  w.scratch_bytes = sb;
-  w.scratch = c.take<char>(sb);
-  w.total = c.off;
-  return w;
+// The forward GEMM y = act(x W^T + b) and the dgrad GEMM gx = (gy W) masked by relu_src > 0, each through the first path that
+// covers it: the weight image when there is one, the raw-weight tensor path (precision 1), the generic pgnn_linear_*.  Only the
+// tensor paths run the epilogue hooks `hk`; *hooked (when given) says whether one did.
+int linear_fwd(const Img& im, const float* x, int64_t ldx, const float* W, const float* b, int64_t M, int64_t N, int64_t K, int relu,
+               float* y, int64_t ldy, int precision, cudaStream_t st, const PgnnGemmHooks* hk = nullptr, bool* hooked = nullptr) {
+  int rc = PGNN_EUNSUPPORTED;
+  if (im.w) rc = pgnn_tc_linear_fwd_img(x, ldx, im.w, im.rows, im.k, b, M, N, K, relu, y, ldy, st, hk);
+  if (rc == PGNN_EUNSUPPORTED && precision == 1) rc = pgnn_tc_linear_fwd(x, ldx, W, b, M, N, K, relu, y, ldy, st, hk);
+  if (hooked) *hooked = rc == PGNN_OK;
+  if (rc == PGNN_EUNSUPPORTED) rc = pgnn_linear_fwd(x, ldx, W, b, M, N, K, relu, y, ldy, precision, st);
+  return rc;
 }
 
-// Weight-gradient GEMMs on a side stream.  They only feed the gradient buffer (GIN: wgrad2 needs gz2, z1 and wgrad1 needs gz1,
-// aggr; conv types: one wgrad on gxl), so on their own stream they run under the next layer's BatchNorm sweeps, attention and
-// gathers (LSU / L2-bound kernels that leave the tensor pipe and most of shared memory idle) instead of in front of them.
-// Ordering is by events; the wgrad operands are double-buffered by layer parity so the main stream never overwrites an operand
-// a pending wgrad still reads.  ready[k][parity] / done[k][parity]: wgrad k's operand is written / wgrad k has finished (GIN
-// uses k = 0 for wgrad2, 1 for wgrad1; the conv types k = 0).  One context per (device, main stream) serves every type.
-// PGNN_WGRAD_STREAM=0 disables.
+int linear_bwd_x(const Img& im, const float* gy, int64_t ldgy, const float* W, int64_t M, int64_t N, int64_t K, const float* relu_src,
+                 int64_t ldr, float* gx, int64_t ldgx, int precision, cudaStream_t st, const PgnnGemmHooks* hk, bool* hooked) {
+  int rc = PGNN_EUNSUPPORTED;
+  if (im.w) rc = pgnn_tc_linear_bwd_x_img(gy, ldgy, im.w, im.rows, im.k, M, N, K, relu_src, ldr, gx, ldgx, st, hk);
+  if (rc == PGNN_EUNSUPPORTED && precision == 1) rc = pgnn_tc_linear_bwd_x(gy, ldgy, W, M, N, K, relu_src, ldr, gx, ldgx, st, hk);
+  *hooked = rc == PGNN_OK;
+  if (rc == PGNN_EUNSUPPORTED) rc = pgnn_linear_bwd_x(gy, ldgy, W, M, N, K, relu_src, ldr, gx, ldgx, precision, st);
+  return rc;
+}
+
+// A Linear (no ReLU) whose tensor-path epilogue also accumulates the BatchNorm batch sums of y into acc [2][N] (fp64 atomics on
+// a zeroed acc).  acc == nullptr, precision 0 or a shape no tensor path covers: a plain Linear with fused = false, and the
+// caller computes the statistics itself.
+int linear_bn_stats(double* acc, const Img& im, const float* x, int64_t ldx, const float* W, const float* b, int64_t M, int64_t N,
+                    int64_t K, float* y, int64_t ldy, int precision, cudaStream_t st, bool& fused) {
+  fused = false;
+  if (!acc || precision != 1) return linear_fwd(im, x, ldx, W, b, M, N, K, 0, y, ldy, precision, st);
+  PGNN_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * 2 * N, st));
+  PgnnGemmHooks hk;
+  hk.stats = acc;
+  return linear_fwd(im, x, ldx, W, b, M, N, K, 0, y, ldy, precision, st, &hk, &fused);
+}
+
+// The finalisation of layer l's BatchNorm from the sums a fused Linear left in acc, for the consumer kernel that applies it: it
+// also updates the running state and saves the batch mean / invstd for the backward.
+PgnnBnFold bn_fold(const BnRun& bn, int64_t l, double* acc, const float* gamma, const float* beta, float* save_mean, float* save_invstd,
+                   int64_t rows) {
+  PgnnBnFold f{};
+  f.acc = acc; f.gamma = gamma; f.beta = beta;
+  f.running_mean = bn.rm(l); f.running_var = bn.rv(l); f.nbt = bn.nb(l);
+  f.save_mean = save_mean; f.save_invstd = save_invstd;
+  f.momentum = bn.momentum; f.eps = bn.eps; f.set_rows((int)rows);
+  return f;
+}
+
+// Weight-gradient GEMMs on a side stream.  They only feed the gradient buffer, so on their own stream they run under the next
+// layer's BatchNorm sweeps, attention and gathers (LSU / L2-bound kernels that leave the tensor pipe and most of shared memory
+// idle) instead of in front of them.  One context per (device, main stream) serves every type; PGNN_WGRAD_STREAM=0 disables.
+// The operands are double-buffered by layer parity so the main stream never overwrites one a pending wgrad still reads.  Event
+// pair k (GIN: 0 = the wgrad of the layer's last Linear, 1 = of its first; the conv types: 0) of parity par orders them:
+//   - before it writes layer l's operand of wgrad k, the main stream waits for done[k][l & 1] (layer l+2's wgrad k is through);
+//   - side_wgrad records ready[k][l & 1] on the main stream, and the side stream waits for it before the wgrad;
+//   - the side stream records done[k][l & 1] after it;
+//   - a wgrad the tensor path does not cover joins the side stream into the main stream and runs there;
+//   - every backward joins the side stream into the main stream before the embedding gradients (join_side).
 struct SideCtx {
   cudaStream_t side = nullptr;
   cudaEvent_t ready[2][2] = {}, done[2][2] = {}, join = nullptr;
@@ -360,22 +430,46 @@ int join_side(const SideCtx* sc, cudaStream_t st) {
   return PGNN_OK;
 }
 
+// the main stream waits until layer l+2's wgrad k has finished reading the operand copy of parity par
+int side_wait(const SideCtx* sc, cudaStream_t st, int k, int par) {
+  if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[k][par], 0));
+  return PGNN_OK;
+}
+
+// One weight-gradient GEMM: gw [Nout, K] = gy^T x and gb = the column sums of gy (gb may be null), ordered as SideCtx describes
+int side_wgrad(const SideCtx* sc, cudaStream_t st, int k, int par, int precision, const float* gy, int64_t ldgy, const float* x,
+               int64_t ldx, int64_t M, int64_t Nout, int64_t K, float* gw, float* gb, float* wpart, int64_t wpart_floats) {
+  cudaStream_t wst = sc ? sc->side : st;
+  if (sc) {
+    PGNN_CUDA(cudaEventRecord(sc->ready[k][par], st));
+    PGNN_CUDA(cudaStreamWaitEvent(wst, sc->ready[k][par], 0));
+  }
+  int rc = PGNN_EUNSUPPORTED;
+  if (precision == 1) rc = pgnn_tc_linear_bwd_w_ws(gy, ldgy, x, ldx, M, Nout, K, gw, gb, wpart, wpart_floats, wst);
+  if (rc == PGNN_EUNSUPPORTED) {
+    if (sc) TRY(join_side(sc, st));
+    return pgnn_linear_bwd_w(gy, ldgy, x, ldx, M, Nout, K, gw, gb, precision, st);
+  }
+  if (rc == PGNN_OK && sc) PGNN_CUDA(cudaEventRecord(sc->done[k][par], wst));
+  return rc;
+}
+
 // Graph preparation, the per-node bond summary S (not for GAT, whose kernels read the bond codes per edge), the atom embedding
 // and, for the tensor-path backward, the one-hot atom-code rows.
 int forward_prologue(int type, const Front& f, const void* const* params, const int64_t* x, const int64_t* edge_index,
                      const int64_t* edge_attr, int64_t N, int64_t E, int64_t D, int training, int precision, void* scratch,
-                     int64_t scratch_bytes, void* stream) {
-  TRY(pgnn_graph_prep(edge_index, E, N, f.rowptr_t, f.nbr_t, f.eid_t, f.rowptr_s, f.nbr_s, f.eid_s, scratch, scratch_bytes, stream));
-  if (type == PGNN_CONV_GCN) TRY(pgnn_gcn_dinv(f.rowptr_t, N, f.dinv, stream));
-  if (type != PGNN_CONV_GAT) TRY(pgnn_chem_edge_summary(edge_attr, f.rowptr_t, f.nbr_t, f.eid_t, N, agg_mode(type), f.dinv, f.S, stream));
-  TRY(pgnn_chem_embed_fwd(x, (const float*)params[P_XEMB1], kAtomRows, (const float*)params[P_XEMB2], kChiralRows, N, D, f.h0, D, stream));
-  if (training && precision == 1) TRY(pgnn_internal_chem_onehot(x, N, kAtomRows, kChiralRows, f.onehot, kOneHotLd, as_stream(stream)));
+                     int64_t scratch_bytes, cudaStream_t st) {
+  TRY(pgnn_graph_prep(edge_index, E, N, f.rowptr_t, f.nbr_t, f.eid_t, f.rowptr_s, f.nbr_s, f.eid_s, scratch, scratch_bytes, st));
+  if (type == PGNN_CONV_GCN) TRY(pgnn_gcn_dinv(f.rowptr_t, N, f.dinv, st));
+  if (type != PGNN_CONV_GAT) TRY(pgnn_chem_edge_summary(edge_attr, f.rowptr_t, f.nbr_t, f.eid_t, N, agg_mode(type), f.dinv, f.S, st));
+  TRY(pgnn_chem_embed_fwd(x, (const float*)params[P_XEMB1], kAtomRows, (const float*)params[P_XEMB2], kChiralRows, N, D, f.h0, D, st));
+  if (training && precision == 1) TRY(pgnn_internal_chem_onehot(x, N, kAtomRows, kChiralRows, f.onehot, kOneHotLd, st));
   return PGNN_OK;
 }
 
-// Backward tail of every type: the side stream's last wgrad (and its use of the split-K workspace) joins the main stream, then
-// the embedding tables: [120 + 3, D] = onehot^T . gh as a split-K weight-gradient GEMM (the two tables are adjacent in the flat
-// layout); the vector-atomics kernel is the FFMA-precision path and the fallback.
+// Backward tail of every chem type: the side stream's last wgrad (and its use of the split-K workspace) joins the main stream,
+// then the embedding tables: [120 + 3, D] = onehot^T . gh as a split-K weight-gradient GEMM (the two tables are adjacent in the
+// flat layout); the vector-atomics kernel is the FFMA-precision path and the fallback.
 int embed_backward(const SideCtx* sc, const Front& f, const float* gh, const int64_t* x, int64_t N, int64_t D, int precision,
                    float* grads, const int64_t* off, float* wpart, int64_t wpart_floats, cudaStream_t st) {
   if (sc) TRY(join_side(sc, st));
@@ -388,26 +482,14 @@ int embed_backward(const SideCtx* sc, const Front& f, const float* gh, const int
   return rc;
 }
 
-int gin_forward(const void* const* params, void* const* bn_running_mean, void* const* bn_running_var, void* const* bn_num_batches_tracked,
-                const int64_t* x, const int64_t* edge_index, const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D,
-                int training, float momentum, float eps, const Drops& drops, int precision, float* node_rep, int64_t ld_out,
-                void* workspace, int64_t workspace_bytes, void* stream) {
-  PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && bn_running_mean && bn_running_var && workspace);
-  PGNN_CHECK_ARG(N == 0 || (x && node_rep));
-  if (workspace_bytes < pgnn_chem_gin_workspace_bytes(N, E, L, D)) return PGNN_EWORKSPACE;
-  if (N == 0) return PGNN_OK;
-  GinWs w = carve_gin(workspace, N, E, L, D);
-  TRY(forward_prologue(kGin, w, params, x, edge_index, edge_attr, N, E, D, training, precision, w.scratch, w.scratch_bytes, stream));
-  cudaStream_t st = as_stream(stream);
+int gin_forward(const void* const* params, const BnRun& bn, int training, const Drops& drops, int precision, float* node_rep,
+                int64_t ld_out, int64_t N, int64_t L, int64_t D, const GinWs& w, cudaStream_t st) {
   GinImages im;
   if (precision == 1) TRY(pack_gin_images(w, params, L, D, false, st, im));
-  const int64_t wide_r = GinImages::rows_pad(2 * D), wide_k = GinImages::k_pad(D);      // mlp.0.weight: 2D rows, reduction D
-  const int64_t narrow_r = GinImages::rows_pad(D), narrow_k = GinImages::k_pad(2 * D);  // mlp.2.weight: D rows, reduction 2D
   const float* h = w.h0;            // input rows of the current layer (pre-affine)
   const float *in_scale = nullptr, *in_shift = nullptr;
   PgnnBnFold fold;                  // pending BatchNorm finalisation of the previous layer (folded into this layer's gather)
   bool have_fold = false;
-  double* const bn_acc = w.bn_acc;  // [L][2][D] fp64 sums
   for (int64_t l = 0; l < L; ++l) {
     const void* const* p = params + P_LAYER0 + l * L_COUNT;
     float* aggr = w.aggr + l * N * D;
@@ -417,48 +499,20 @@ int gin_forward(const void* const* params, void* const* bn_running_mean, void* c
     const PgnnDropout drop_in = drops.at(l > 0 ? l - 1 : 0), drop_out = drops.at(l);  // the previous layer's mask, this layer's
     // gather (the previous layer's BatchNorm + ReLU + dropout applied on load) + GEMM1
     TRY(pgnn_internal_aggregate_fwd(h, D, in_scale, in_shift, in_scale != nullptr || have_fold, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_SUM,
-                                    nullptr, w.S, 9, (const float*)p[L_ET1], (const float*)p[L_ET2], 6, 0, aggr, D, as_stream(stream),
+                                    nullptr, w.S, kChemQ, (const float*)p[L_ET1], (const float*)p[L_ET2], kChemQSplit, 0, aggr, D, st,
                                     have_fold ? &fold : nullptr, l > 0 ? &drop_in : nullptr));
-    int rc1 = im.on ? pgnn_tc_linear_fwd_img(aggr, D, im.wide(l), wide_r, wide_k, (const float*)p[L_B1], N, 2 * D, D, 1, z1, 2 * D, st,
-                                             nullptr)
-                    : PGNN_EUNSUPPORTED;
-    if (rc1 == PGNN_EUNSUPPORTED)
-      rc1 = pgnn_linear_fwd(aggr, D, (const float*)p[L_W1], (const float*)p[L_B1], N, 2 * D, D, 1, z1, 2 * D, precision, stream);
-    if (rc1 != PGNN_OK) return rc1;
+    TRY(linear_fwd(im.wide(l), aggr, D, (const float*)p[L_W1], (const float*)p[L_B1], N, 2 * D, D, 1, z1, 2 * D, precision, st));
     have_fold = false;
-    // GEMM2; on the tensor path its epilogue also accumulates the BatchNorm batch statistics of z2 (fp64 atomics)
-    bool stats_fused = false;
-    double* acc = bn_acc + l * 2 * D;
-    if (training && precision == 1) {
-      PGNN_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * 2 * D, as_stream(stream)));
-      PgnnGemmHooks hk;
-      hk.stats = acc;
-      int rc = im.on ? pgnn_tc_linear_fwd_img(z1, 2 * D, im.narrow(l), narrow_r, narrow_k, (const float*)p[L_B2], N, D, 2 * D, 0, z2, D,
-                                              st, &hk)
-                     : PGNN_EUNSUPPORTED;
-      if (rc == PGNN_EUNSUPPORTED)
-        rc = pgnn_tc_linear_fwd(z1, 2 * D, (const float*)p[L_W2], (const float*)p[L_B2], N, D, 2 * D, 0, z2, D, st, &hk);
-      if (rc == PGNN_OK) stats_fused = true;
-      else if (rc != PGNN_EUNSUPPORTED) return rc;
-    }
-    if (!stats_fused) {
-      int rc = im.on && !training ? pgnn_tc_linear_fwd_img(z1, 2 * D, im.narrow(l), narrow_r, narrow_k, (const float*)p[L_B2], N, D,
-                                                           2 * D, 0, z2, D, st, nullptr)
-                                  : PGNN_EUNSUPPORTED;
-      if (rc == PGNN_EUNSUPPORTED)
-        rc = pgnn_linear_fwd(z1, 2 * D, (const float*)p[L_W2], (const float*)p[L_B2], N, D, 2 * D, 0, z2, D, precision, stream);
-      if (rc != PGNN_OK) return rc;
-    }
-    if (training && stats_fused) {
+    // GEMM2; in training on the tensor path its epilogue also accumulates the BatchNorm batch statistics of z2
+    double* acc = w.bn_acc + l * 2 * D;
+    bool stats_fused;
+    TRY(linear_bn_stats(training ? acc : nullptr, im.narrow(l), z1, 2 * D, (const float*)p[L_W2], (const float*)p[L_B2], N, D, 2 * D, z2, D,
+                        precision, st, stats_fused));
+    if (stats_fused) {
       // no finalize launch: the consumer (next layer's gather, or the final apply) derives scale/shift from the sums
-      fold = PgnnBnFold{};
-      fold.acc = acc; fold.gamma = (const float*)p[L_GAMMA]; fold.beta = (const float*)p[L_BETA];
-      fold.running_mean = (float*)bn_running_mean[l]; fold.running_var = (float*)bn_running_var[l];
-      fold.nbt = bn_num_batches_tracked ? (int64_t*)bn_num_batches_tracked[l] : nullptr;
-      fold.save_mean = w.mean + l * D; fold.save_invstd = w.invstd + l * D;
-      fold.momentum = momentum; fold.eps = eps; fold.set_rows((int)N);
+      fold = bn_fold(bn, l, acc, (const float*)p[L_GAMMA], (const float*)p[L_BETA], w.mean + l * D, w.invstd + l * D, N);
       if (last) {
-        TRY(pgnn_internal_bn_apply_fold(z2, D, N, D, fold, 0, node_rep, ld_out, as_stream(stream), &drop_out));
+        TRY(pgnn_internal_bn_apply_fold(z2, D, N, D, fold, 0, node_rep, ld_out, st, &drop_out));
       } else {
         have_fold = true;
       }
@@ -466,18 +520,17 @@ int gin_forward(const void* const* params, void* const* bn_running_mean, void* c
       in_scale = in_shift = nullptr;
     } else if (training) {
       // statistics only for inner layers (applied on load by the next gather); the last layer materialises node_rep
-      TRY(pgnn_internal_bn_fwd_train(z2, D, N, D, (const float*)p[L_GAMMA], (const float*)p[L_BETA], (float*)bn_running_mean[l],
-                                     (float*)bn_running_var[l], bn_num_batches_tracked ? (int64_t*)bn_num_batches_tracked[l] : nullptr,
-                                     momentum, eps, 0, last ? node_rep : nullptr, ld_out, w.mean + l * D, w.invstd + l * D, w.scale + l * D,
-                                     w.shift + l * D, w.scratch, w.scratch_bytes, stream, &drop_out));
+      TRY(pgnn_internal_bn_fwd_train(z2, D, N, D, (const float*)p[L_GAMMA], (const float*)p[L_BETA], bn.rm(l), bn.rv(l), bn.nb(l),
+                                     bn.momentum, bn.eps, 0, last ? node_rep : nullptr, ld_out, w.mean + l * D, w.invstd + l * D,
+                                     w.scale + l * D, w.shift + l * D, w.scratch, w.scratch_bytes, st, &drop_out));
       h = z2;
       in_scale = w.scale + l * D;
       in_shift = w.shift + l * D;
     } else {
       // eval: plain BN(+ReLU) pass with the running statistics, ping-ponging between two spare buffers
       float* y = last ? node_rep : ((l & 1) ? w.gz2 : w.gaggr);
-      TRY(pgnn_bn_fwd_eval(z2, D, N, D, (const float*)p[L_GAMMA], (const float*)p[L_BETA], (const float*)bn_running_mean[l],
-                           (const float*)bn_running_var[l], eps, !last, y, last ? ld_out : D, stream));
+      TRY(pgnn_bn_fwd_eval(z2, D, N, D, (const float*)p[L_GAMMA], (const float*)p[L_BETA], bn.rm(l), bn.rv(l), bn.eps, !last, y,
+                           last ? ld_out : D, st));
       h = y;
       in_scale = in_shift = nullptr;
     }
@@ -485,30 +538,14 @@ int gin_forward(const void* const* params, void* const* bn_running_mean, void* c
   return PGNN_OK;
 }
 
-int gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x, int64_t N, int64_t E, int64_t L,
-                 int64_t D, const Drops& drops, int precision, float* grads, void* workspace, int64_t workspace_bytes, void* stream) {
-  PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && grads && workspace);
-  if (workspace_bytes < pgnn_chem_gin_workspace_bytes(N, E, L, D)) return PGNN_EWORKSPACE;
-  const int64_t count = grad_layout(kGin, L, D, nullptr);
-  std::vector<int64_t> offsets(count + 1);
-  const int64_t* off = offsets.data();
-  grad_layout(kGin, L, D, offsets.data());
-  cudaStream_t st = as_stream(stream);
-  if (N == 0) {
-    PGNN_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * off[count], st));
-    return PGNN_OK;
-  }
-  PGNN_CHECK_ARG(g_node_rep && x);
-  GinWs w = carve_gin(workspace, N, E, L, D);
+int gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x, int64_t N, int64_t L, int64_t D,
+                 const Drops& drops, int precision, float* grads, const int64_t* off, const GinWs& w, cudaStream_t st) {
   // images of the transposed MLP weights: the dgrad B operands, reduction-contiguous and already split
   GinImages im;
   if (precision == 1) TRY(pack_gin_images(w, params, L, D, true, st, im));
-  const int64_t wide_r = GinImages::rows_pad(2 * D), wide_k = GinImages::k_pad(D);      // mlp.2.weight^T: 2D rows, reduction D
-  const int64_t narrow_r = GinImages::rows_pad(D), narrow_k = GinImages::k_pad(2 * D);  // mlp.0.weight^T: D rows, reduction 2D
   const float* gy = g_node_rep;
   int64_t ldgy = ldg;
   SideCtx* sc = precision == 1 ? side_ctx(st) : nullptr;
-  cudaStream_t wst = sc ? sc->side : st;   // the stream of the weight-gradient GEMMs
   for (int64_t l = L - 1; l >= 0; --l) {
     const void* const* p = params + P_LAYER0 + l * L_COUNT;
     const int64_t* o = off + P_LAYER0 + l * L_COUNT;
@@ -521,196 +558,32 @@ int gin_backward(const void* const* params, const float* g_node_rep, int64_t ldg
     float* gz1 = w.gz1 + (sc ? par * N * 2 * D : 0);
     // BatchNorm (dropout mask regenerated, ReLU mask recomputed from z2) backward; the same pass leaves colsum(gz2) = gradient
     // of mlp.2.bias
-    if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad2 has finished reading this copy
+    TRY(side_wait(sc, st, 0, par));
     const PgnnDropout drop = drops.at(l);
     TRY(pgnn_internal_bn_bwd(gy, ldgy, z2, D, N, D, (const float*)p[L_GAMMA], (const float*)p[L_BETA], w.mean + l * D,
                              w.invstd + l * D, !last, gz2, D, grads + o[L_GAMMA], grads + o[L_BETA], grads + o[L_B2],
                              w.scratch, w.scratch_bytes, st, &drop));
-    // MLP backward.  On the tensor path the dgrad epilogues carry the column reductions that would otherwise be
-    // passes of their own: colsum(gz1) = gradient of mlp.0.bias, and S^T gaggr = gradient of the two bond tables.
-    bool fused = false;
-    if (precision == 1) {
-      if (sc) {
-        PGNN_CUDA(cudaEventRecord(sc->ready[0][par], st));
-        PGNN_CUDA(cudaStreamWaitEvent(wst, sc->ready[0][par], 0));
-      }
-      int rc = pgnn_tc_linear_bwd_w_ws(gz2, D, z1, 2 * D, N, D, 2 * D, grads + o[L_W2], nullptr, w.wpart, w.wpart_floats, wst);
-      if (rc == PGNN_OK) {
-        if (sc) {
-          PGNN_CUDA(cudaEventRecord(sc->done[0][par], wst));
-          PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[1][par], 0));  // layer l+2's wgrad1 has finished reading gz1[par]
-        }
-        PGNN_CUDA(cudaMemsetAsync(grads + o[L_B1], 0, sizeof(float) * 2 * D, st));
-        PgnnGemmHooks h1;
-        h1.colsum = grads + o[L_B1];
-        rc = im.on ? pgnn_tc_linear_bwd_x_img(gz2, D, im.wide(l), wide_r, wide_k, N, D, 2 * D, z1, 2 * D, gz1, 2 * D, st, &h1)
-                   : PGNN_EUNSUPPORTED;
-        if (rc == PGNN_EUNSUPPORTED)
-          rc = pgnn_tc_linear_bwd_x(gz2, D, (const float*)p[L_W2], N, D, 2 * D, z1, 2 * D, gz1, 2 * D, st, &h1);
-        if (rc != PGNN_OK) return rc;
-        if (sc) {
-          PGNN_CUDA(cudaEventRecord(sc->ready[1][par], st));
-          PGNN_CUDA(cudaStreamWaitEvent(wst, sc->ready[1][par], 0));
-        }
-        rc = pgnn_tc_linear_bwd_w_ws(gz1, 2 * D, aggr, D, N, 2 * D, D, grads + o[L_W1], nullptr, w.wpart, w.wpart_floats, wst);
-        if (rc != PGNN_OK) return rc;
-        if (sc) PGNN_CUDA(cudaEventRecord(sc->done[1][par], wst));
-        PGNN_CUDA(cudaMemsetAsync(grads + o[L_ET1], 0, sizeof(float) * 9 * D, st));  // the two tables are adjacent in the layout
-        PgnnGemmHooks h2;
-        h2.S = w.S; h2.Q = 9; h2.gT = grads + o[L_ET1]; h2.gT2 = grads + o[L_ET2]; h2.q_split = 6; h2.ldt = D;
-        rc = im.on ? pgnn_tc_linear_bwd_x_img(gz1, 2 * D, im.narrow(l), narrow_r, narrow_k, N, 2 * D, D, nullptr, 0, w.gaggr, D, st, &h2)
-                   : PGNN_EUNSUPPORTED;
-        if (rc == PGNN_EUNSUPPORTED)
-          rc = pgnn_tc_linear_bwd_x(gz1, 2 * D, (const float*)p[L_W1], N, 2 * D, D, nullptr, 0, w.gaggr, D, st, &h2);
-        if (rc != PGNN_OK) return rc;
-        fused = true;
-      } else if (rc != PGNN_EUNSUPPORTED) {
-        return rc;
-      }
-    }
-    if (!fused) {
-      if (sc) TRY(join_side(sc, st));  // an unsupported shape on the tensor path: everything on the caller's stream from here on
-      TRY(pgnn_linear_bwd_w(gz2, D, z1, 2 * D, N, D, 2 * D, grads + o[L_W2], nullptr, precision, stream));
-      TRY(pgnn_linear_bwd_x(gz2, D, (const float*)p[L_W2], N, D, 2 * D, z1, 2 * D, gz1, 2 * D, precision, stream));
-      TRY(pgnn_linear_bwd_w(gz1, 2 * D, aggr, D, N, 2 * D, D, grads + o[L_W1], grads + o[L_B1], precision, stream));
-      TRY(pgnn_linear_bwd_x(gz1, 2 * D, (const float*)p[L_W1], N, 2 * D, D, nullptr, 0, w.gaggr, D, precision, stream));
-      // bond tables: gT = S^T gaggr, rows 0..5 -> edge_embedding1, 6..8 -> edge_embedding2
-      PGNN_CUDA(cudaMemsetAsync(grads + o[L_ET1], 0, sizeof(float) * 9 * D, st));
-      TRY(pgnn_internal_edge_table_bwd2(w.S, 9, w.gaggr, D, 0, N, (int)D, grads + o[L_ET1], D, grads + o[L_ET2], 6, st));
-    }
+    // MLP backward.  On the tensor path the dgrad epilogues carry the column reductions that would otherwise be passes of
+    // their own: colsum(gz1) = gradient of mlp.0.bias, and S^T gaggr = gradient of the two bond tables.  Where a dgrad falls
+    // back, wgrad1 computes the bias gradient and a separate pass the tables'.
+    TRY(side_wgrad(sc, st, 0, par, precision, gz2, D, z1, 2 * D, N, D, 2 * D, grads + o[L_W2], nullptr, w.wpart, w.wpart_floats));
+    TRY(side_wait(sc, st, 1, par));
+    PGNN_CUDA(cudaMemsetAsync(grads + o[L_B1], 0, sizeof(float) * 2 * D, st));
+    PgnnGemmHooks h1;
+    h1.colsum = grads + o[L_B1];
+    bool b1_done;
+    TRY(linear_bwd_x(im.wide(l), gz2, D, (const float*)p[L_W2], N, D, 2 * D, z1, 2 * D, gz1, 2 * D, precision, st, &h1, &b1_done));
+    TRY(side_wgrad(sc, st, 1, par, precision, gz1, 2 * D, aggr, D, N, 2 * D, D, grads + o[L_W1], b1_done ? nullptr : grads + o[L_B1],
+                   w.wpart, w.wpart_floats));
+    PGNN_CUDA(cudaMemsetAsync(grads + o[L_ET1], 0, sizeof(float) * kChemQ * D, st));  // the two tables are adjacent in the layout
+    PgnnGemmHooks h2;
+    h2.S = w.S; h2.Q = kChemQ; h2.gT = grads + o[L_ET1]; h2.gT2 = grads + o[L_ET2]; h2.q_split = kChemQSplit; h2.ldt = D;
+    bool et_done;
+    TRY(linear_bwd_x(im.narrow(l), gz1, 2 * D, (const float*)p[L_W1], N, 2 * D, D, nullptr, 0, w.gaggr, D, precision, st, &h2, &et_done));
+    if (!et_done)
+      TRY(pgnn_internal_edge_table_bwd2(w.S, kChemQ, w.gaggr, D, 0, N, (int)D, grads + o[L_ET1], D, grads + o[L_ET2], kChemQSplit, st));
     // transpose-graph gather: gradient w.r.t. this layer's input rows
-    TRY(pgnn_aggregate_bwd(w.gaggr, D, N, D, w.rowptr_s, w.nbr_s, PGNN_AGG_SUM, nullptr, w.rowptr_t, w.gh, D, stream));
-    gy = w.gh;
-    ldgy = D;
-  }
-  return embed_backward(sc, w, w.gh, x, N, D, precision, grads, off, w.wpart, w.wpart_floats, st);
-}
-
-int conv_forward(int conv_type, const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
-                 void* const* bn_num_batches_tracked, const int64_t* x, const int64_t* edge_index, const int64_t* edge_attr, int64_t N,
-                 int64_t E, int64_t L, int64_t D, int training, float momentum, float eps, const Drops& drops, int precision,
-                 float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes, void* stream) {
-  PGNN_CHECK_ARG(valid_conv(conv_type) && N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && bn_running_mean && bn_running_var &&
-                 workspace);
-  PGNN_CHECK_ARG(N == 0 || (x && node_rep));
-  PGNN_CHECK_ARG(E == 0 || (edge_index && edge_attr));
-  if (workspace_bytes < pgnn_chem_conv_workspace_bytes(conv_type, N, E, L, D)) return PGNN_EWORKSPACE;
-  if (N == 0) return PGNN_OK;
-  cudaStream_t st = as_stream(stream);
-  const bool gat = conv_type == PGNN_CONV_GAT;
-  const int64_t HD = gat ? kHeads * D : D;
-  const int PL = layer_params(conv_type);
-  ConvWs w = carve_conv(workspace, conv_type, N, E, L, D);
-  TRY(forward_prologue(conv_type, w, params, x, edge_index, edge_attr, N, E, D, training, precision, w.scratch, w.scratch_bytes, stream));
-  const float* h = w.h0;
-  for (int64_t l = 0; l < L; ++l) {
-    const void* const* p = params + P_LAYER0 + l * PL;
-    const bool last = l == L - 1;
-    float* xl = w.xl + l * N * HD;
-    float* z = w.z + l * N * D;
-    float* hout = last ? node_rep : w.hout + l * N * D;
-    const int64_t ldh = last ? ld_out : D;
-    TRY(pgnn_linear_fwd(h, D, (const float*)p[gat ? A_W : G_W], (const float*)p[gat ? A_B : G_B], N, HD, D, 0, xl, HD, precision, stream));
-    if (gat) {
-      float* T = w.T + l * 9 * HD;  // the kernels index one [9, H*D] table: rows 0..5 bond type, 6..8 bond direction
-      PGNN_CUDA(cudaMemcpyAsync(T, p[A_ET1], sizeof(float) * 6 * HD, cudaMemcpyDeviceToDevice, st));
-      PGNN_CUDA(cudaMemcpyAsync(T + 6 * HD, p[A_ET2], sizeof(float) * 3 * HD, cudaMemcpyDeviceToDevice, st));
-      TRY(pgnn_gat_fwd(xl, N, kHeads, D, (const float*)p[A_ATT], T, 0, edge_attr, w.rowptr_t, w.nbr_t, w.eid_t, E, (const float*)p[A_BIAS], kSlope,
-                       w.alpha + l * (E + N) * kHeads, w.pq + l * N * kHeads * 2, z, D, stream));
-    } else if (conv_type == PGNN_CONV_GCN) {
-      TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_GCN, w.dinv, w.S, 9, (const float*)p[G_ET1],
-                                      (const float*)p[G_ET2], 6, 0, z, D, st, nullptr, nullptr));
-    } else {
-      // mean aggregation into the backward scratch `gz` (only its normalised rows and their norms are needed later)
-      TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_MEAN, nullptr, w.S, 9, (const float*)p[G_ET1],
-                                      (const float*)p[G_ET2], 6, 0, w.gz, D, st, nullptr, nullptr));
-      TRY(pgnn_l2norm_fwd(w.gz, D, N, D, z, D, w.nrm + l * N, stream));
-    }
-    const float* gamma = (const float*)p[gat ? A_GAMMA : G_GAMMA];
-    const float* beta = (const float*)p[gat ? A_BETA : G_BETA];
-    if (training) {
-      const PgnnDropout drop = drops.at(l);  // after the ReLU: hout is the next layer's input and its Linear's weight-gradient operand
-      TRY(pgnn_internal_bn_fwd_train(z, D, N, D, gamma, beta, (float*)bn_running_mean[l], (float*)bn_running_var[l],
-                                     bn_num_batches_tracked ? (int64_t*)bn_num_batches_tracked[l] : nullptr, momentum, eps, !last, hout, ldh,
-                                     w.mean + l * D, w.invstd + l * D, nullptr, nullptr, w.scratch, w.scratch_bytes, stream, &drop));
-    } else {
-      TRY(pgnn_bn_fwd_eval(z, D, N, D, gamma, beta, (const float*)bn_running_mean[l], (const float*)bn_running_var[l], eps, !last, hout, ldh, stream));
-    }
-    h = hout;
-  }
-  return PGNN_OK;
-}
-
-int conv_backward(int conv_type, const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x,
-                  const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, const Drops& drops, int precision, float* grads,
-                  void* workspace, int64_t workspace_bytes, void* stream) {
-  PGNN_CHECK_ARG(valid_conv(conv_type) && N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && grads && workspace);
-  if (workspace_bytes < pgnn_chem_conv_workspace_bytes(conv_type, N, E, L, D)) return PGNN_EWORKSPACE;
-  const int64_t count = grad_layout(conv_type, L, D, nullptr);
-  std::vector<int64_t> offsets(count + 1);
-  const int64_t* off = offsets.data();
-  grad_layout(conv_type, L, D, offsets.data());
-  cudaStream_t st = as_stream(stream);
-  const bool gat = conv_type == PGNN_CONV_GAT;
-  const int64_t HD = gat ? kHeads * D : D;
-  const int PL = layer_params(conv_type);
-  if (N == 0) {
-    PGNN_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * off[count], st));
-    return PGNN_OK;
-  }
-  PGNN_CHECK_ARG(g_node_rep && x && (E == 0 || edge_attr));
-  ConvWs w = carve_conv(workspace, conv_type, N, E, L, D);
-  const float* gy = g_node_rep;
-  int64_t ldgy = ldg;
-  SideCtx* sc = precision == 1 ? side_ctx(st) : nullptr;
-  cudaStream_t wst = sc ? sc->side : st;
-  for (int64_t l = L - 1; l >= 0; --l) {
-    const void* const* p = params + P_LAYER0 + l * PL;
-    const int64_t* o = off + P_LAYER0 + l * PL;
-    const bool last = l == L - 1;
-    const int par = (int)(l & 1);
-    const float* xl = w.xl + l * N * HD;
-    const float* z = w.z + l * N * D;
-    const float* hin = l == 0 ? w.h0 : w.hout + (l - 1) * N * D;
-    float* gxl = w.gxl + (sc ? par * N * HD : 0);
-    const float* gamma = (const float*)p[gat ? A_GAMMA : G_GAMMA];
-    const float* beta = (const float*)p[gat ? A_BETA : G_BETA];
-    const PgnnDropout drop = drops.at(l);
-    TRY(pgnn_internal_bn_bwd(gy, ldgy, z, D, N, D, gamma, beta, w.mean + l * D, w.invstd + l * D, !last, w.gz, D,
-                             grads + o[gat ? A_GAMMA : G_GAMMA], grads + o[gat ? A_BETA : G_BETA], nullptr, w.scratch, w.scratch_bytes, st,
-                             &drop));
-    if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad has finished reading this copy of gxl
-    if (gat) {
-      // gT [9, HD] lands on the two adjacent bond-table gradients
-      TRY(pgnn_gat_bwd(w.gz, D, xl, N, kHeads, D, (const float*)p[A_ATT], w.T + l * 9 * HD, 0, edge_attr, w.rowptr_t, w.nbr_t, w.eid_t, w.rowptr_s,
-                       w.nbr_s, w.eid_s, E, kSlope, w.alpha + l * (E + N) * kHeads, w.pq + l * N * kHeads * 2, gxl, grads + o[A_ATT],
-                       grads + o[A_ET1], grads + o[A_BIAS], w.scratch, w.scratch_bytes, stream));
-    } else {
-      const float* ga = w.gz;
-      if (conv_type == PGNN_CONV_SAGE) {
-        TRY(pgnn_l2norm_bwd(w.gz, D, z, D, w.nrm + l * N, N, D, w.ga, D, stream));
-        ga = w.ga;
-      }
-      PGNN_CUDA(cudaMemsetAsync(grads + o[G_ET1], 0, sizeof(float) * 9 * D, st));
-      TRY(pgnn_internal_edge_table_bwd2(w.S, 9, ga, D, 0, N, (int)D, grads + o[G_ET1], D, grads + o[G_ET2], 6, st));
-      TRY(pgnn_aggregate_bwd(ga, D, N, D, w.rowptr_s, w.nbr_s, agg_mode(conv_type), w.dinv, w.rowptr_t, gxl, D, stream));
-    }
-    // Linear backward: weight + bias gradients (side stream), then the input gradient
-    if (sc) {
-      PGNN_CUDA(cudaEventRecord(sc->ready[0][par], st));
-      PGNN_CUDA(cudaStreamWaitEvent(wst, sc->ready[0][par], 0));
-    }
-    int rc = PGNN_EUNSUPPORTED;
-    if (precision == 1)
-      rc = pgnn_tc_linear_bwd_w_ws(gxl, HD, hin, D, N, HD, D, grads + o[gat ? A_W : G_W], grads + o[gat ? A_B : G_B], w.wpart, w.wpart_floats, wst);
-    if (rc == PGNN_EUNSUPPORTED) {
-      if (sc) TRY(join_side(sc, st));
-      rc = pgnn_linear_bwd_w(gxl, HD, hin, D, N, HD, D, grads + o[gat ? A_W : G_W], grads + o[gat ? A_B : G_B], precision, stream);
-    } else if (sc) {
-      PGNN_CUDA(cudaEventRecord(sc->done[0][par], wst));
-    }
-    if (rc != PGNN_OK) return rc;
-    TRY(pgnn_linear_bwd_x(gxl, HD, (const float*)p[gat ? A_W : G_W], N, HD, D, nullptr, 0, w.gh, D, precision, stream));
+    TRY(pgnn_aggregate_bwd(w.gaggr, D, N, D, w.rowptr_s, w.nbr_s, PGNN_AGG_SUM, nullptr, w.rowptr_t, w.gh, D, st));
     gy = w.gh;
     ldgy = D;
   }
@@ -724,13 +597,13 @@ int conv_backward(int conv_type, const void* const* params, const float* g_node_
 // per-node summary S [N, 10] (pgnn_bio_edge_summary) and the table T [10, C] = [W^T ; b]: the forward packs every layer's table in
 // one launch, and the backward scatters every layer's table gradient back as the encoder's weight [C, 9] and bias [C] in one.
 //   GIN        aggr = [sum_j x_j || S.T] (2D wide), then Linear(2D,2D) -> BatchNorm1d(2D) -> ReLU -> Linear(2D,D)
-//   GCN / GraphSAGE / GAT: as for chem, with the bio table (GAT reads the 9 float attributes per edge).
+//   GCN / GraphSAGE / GAT: the chem layer body (conv_forward / conv_backward) with the bio table (GAT reads the 9 float
+//              attributes per edge).
 // There is no outer BatchNorm: every layer but the last is followed by ReLU, then by layer l's dropout mask.  GIN applies both on
 // load in the next layer's gather (and, under dropout, its last layer takes one dropout sweep that writes node_rep); the conv
 // types take one ReLU + dropout sweep per layer that writes the layer's output (bio_act).  The backward runs the matching sweep
 // on the incoming gradient of every layer.
 
-constexpr int kBioQ = 10;       // S columns: the 9 edge attributes + the weight sum that multiplies the encoder bias
 constexpr int kBioEmbRows = 2;  // input_node_embeddings
 constexpr int kMaxPack = 64;    // layers per table-pack launch (their pointers travel as kernel arguments)
 
@@ -741,11 +614,11 @@ enum BioParam {
   BC_W = 0, BC_B, BC_ENC_W, BC_ENC_B, BC_COUNT,                                     // gcn / graphsage
   BA_W = 0, BA_B, BA_ATT, BA_BIAS, BA_ENC_W, BA_ENC_B, BA_COUNT                     // gat
 };
+static_assert(BC_W == CV_W && BC_B == CV_B && BA_W == CV_W && BA_B == CV_B && BA_ATT == CV_ATT && BA_BIAS == CV_BIAS, "bio conv order");
 
 inline int bio_layer_params(int type) { return type == kGin ? BG_COUNT : type == PGNN_CONV_GAT ? BA_COUNT : BC_COUNT; }
 inline int bio_enc_w(int type) { return type == kGin ? BG_ENC_W : type == PGNN_CONV_GAT ? BA_ENC_W : BC_ENC_W; }
 inline int64_t bio_width(int type, int64_t D) { return type == PGNN_CONV_GAT ? kHeads * D : D; }  // C: the edge encoder's width
-bool valid_type(int t) { return t == kGin || valid_conv(t); }
 
 int64_t bio_grad_layout(int type, int64_t L, int64_t D, int64_t* offsets) {
   if (!offsets) return 1 + (int64_t)bio_layer_params(type) * L;
@@ -884,24 +757,20 @@ int bio_pack_tables(int type, const void* const* params, int64_t L, int64_t C, f
   return PGNN_OK;
 }
 
-struct BioGinWs : Front {
+struct BioGinWs : Front, Tail {
   float* T;                      // [L][10][D] packed edge-encoder tables
   double* bn_acc;                // [L][2][2D] fp64 sums of the inner BatchNorm (tensor path)
   float *mean, *invstd;          // [L, 2D]
   float *aggr, *z1, *y1, *z2;    // per layer: gather [N, 2D], Linear 1 [N, 2D], BatchNorm + ReLU [N, 2D], Linear 2 [N, D]
   float *gz2, *gy1, *gz1, *ga;   // backward temporaries; gz2 and gz1 two copies by layer parity (side-stream wgrad operands)
   float *gh, *gT;                // [N, D], [L][10][D]
-  float* wpart;
-  int64_t wpart_floats;
-  void* scratch;
-  int64_t scratch_bytes, total;
 };
 
 BioGinWs carve_bio_gin(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
-  Carve c(base, false);
+  Carve c(base);
   BioGinWs w;
   const int64_t D2 = 2 * D;
-  carve_front(c, w, kGin, N, E, D, kBioQ, 0);
+  carve_front(c, w, true, kGin, N, E, D);
   w.T = c.take<float>(L * kBioQ * D);
   w.bn_acc = c.take<double>(L * 2 * D2);
   w.mean = c.take<float>(L * D2);
@@ -917,60 +786,8 @@ BioGinWs carve_bio_gin(void* base, int64_t N, int64_t E, int64_t L, int64_t D) {
   w.gh = c.take<float>(N * D);
   w.gT = c.take<float>(L * kBioQ * D);
   const int64_t a = pgnn_tc_wgrad_workspace_floats(N, D2, D2), b = pgnn_tc_wgrad_workspace_floats(N, D, D2);
-  w.wpart_floats = a > b ? a : b;
-  w.wpart = c.take<float>(w.wpart_floats);
-  int64_t sb = pgnn_graph_prep_workspace_bytes(N, E);
-  const int64_t bb = pgnn_bn_workspace_bytes(N > 0 ? N : 1, D2);
-  if (bb > sb) sb = bb;
-  w.scratch_bytes = sb;
-  w.scratch = c.take<char>(sb);
-  w.total = c.off;
+  carve_tail(c, w, kGin, N, E, D, a > b ? a : b, D2);
   return w;
-}
-
-struct BioConvWs : Front {
-  float *T, *xl, *z, *hout;    // [L][10][C]; per layer: Linear output [N, C], conv output [N, D], after ReLU + dropout [N, D]
-  float *nrm, *alpha, *pq;     // per layer: SAGE row norms [N]; GAT attention [(E+N), H] and logit halves [N, H, 2]
-  float *gz, *ga, *gxl, *gh;   // backward temporaries [N, D], [N, D], two copies of [N, C] by layer parity, [N, D]
-  float* gT;                   // [L][10][C]
-  float* wpart;
-  int64_t wpart_floats;
-  void* scratch;
-  int64_t scratch_bytes, total;
-};
-
-BioConvWs carve_bio_conv(void* base, int type, int64_t N, int64_t E, int64_t L, int64_t D) {
-  Carve c(base, true);
-  BioConvWs w;
-  const int64_t C = bio_width(type, D);
-  carve_front(c, w, type, N, E, D, kBioQ, 0);
-  w.T = c.take<float>(L * kBioQ * C);
-  w.xl = c.take<float>(L * N * C);
-  w.z = c.take<float>(L * N * D);
-  w.hout = c.take<float>(L * N * D);
-  w.nrm = c.take<float>(type == PGNN_CONV_SAGE ? L * N : 0);
-  w.alpha = c.take<float>(type == PGNN_CONV_GAT ? L * (E + N) * kHeads : 0);
-  w.pq = c.take<float>(type == PGNN_CONV_GAT ? L * N * kHeads * 2 : 0);
-  w.gz = c.take<float>(N * D);
-  w.ga = c.take<float>(N * D);
-  w.gxl = c.take<float>(2 * N * C);
-  w.gh = c.take<float>(N * D);
-  w.gT = c.take<float>(L * kBioQ * C);
-  w.wpart_floats = pgnn_tc_wgrad_workspace_floats(N, C, D);
-  w.wpart = c.take<float>(w.wpart_floats);
-  int64_t sb = pgnn_graph_prep_workspace_bytes(N, E);
-  if (type == PGNN_CONV_GAT) {
-    const int64_t gb = pgnn_gat_bwd_workspace_bytes(N, E, kHeads, D);
-    if (gb > sb) sb = gb;
-  }
-  w.scratch_bytes = sb;
-  w.scratch = c.take<char>(sb);
-  w.total = c.off;
-  return w;
-}
-
-int64_t bio_workspace_bytes(int type, int64_t N, int64_t E, int64_t L, int64_t D) {
-  return type == kGin ? carve_bio_gin(nullptr, N, E, L, D).total : carve_bio_conv(nullptr, type, N, E, L, D).total;
 }
 
 // Graph preparation, the summary S (not for GAT, whose kernels read the attributes per edge), the label embedding and every
@@ -982,26 +799,6 @@ int bio_prologue(int type, const Front& f, float* T, const void* const* params, 
   if (type != PGNN_CONV_GAT) TRY(pgnn_bio_edge_summary(edge_attr, f.rowptr_t, f.nbr_t, f.eid_t, N, agg_mode(type), f.dinv, f.S, st));
   TRY(pgnn_bio_embed_fwd(x, (const float*)params[PB_EMB], N, D, f.h0, D, st));
   return bio_pack_tables(type, params, L, bio_width(type, D), T, st);
-}
-
-// One weight-gradient GEMM of the bio backward: gw [Nout, K] = gy^T x and gb = the column sums of gy (gb may be null), on the side
-// stream when there is one, ordered by the context's event pair k of this layer parity (SideCtx).  A shape the tensor path does
-// not cover runs on the caller's stream once everything on the side stream has finished.
-int side_wgrad(const SideCtx* sc, cudaStream_t st, int k, int par, int precision, const float* gy, int64_t ldgy, const float* x,
-               int64_t ldx, int64_t M, int64_t Nout, int64_t K, float* gw, float* gb, float* wpart, int64_t wpart_floats) {
-  cudaStream_t wst = sc ? sc->side : st;
-  if (sc) {
-    PGNN_CUDA(cudaEventRecord(sc->ready[k][par], st));
-    PGNN_CUDA(cudaStreamWaitEvent(wst, sc->ready[k][par], 0));
-  }
-  int rc = PGNN_EUNSUPPORTED;
-  if (precision == 1) rc = pgnn_tc_linear_bwd_w_ws(gy, ldgy, x, ldx, M, Nout, K, gw, gb, wpart, wpart_floats, wst);
-  if (rc == PGNN_EUNSUPPORTED) {
-    if (sc) TRY(join_side(sc, st));
-    return pgnn_linear_bwd_w(gy, ldgy, x, ldx, M, Nout, K, gw, gb, precision, st);
-  }
-  if (rc == PGNN_OK && sc) PGNN_CUDA(cudaEventRecord(sc->done[k][par], wst));
-  return rc;
 }
 
 // Backward tail of every bio type: the side stream joins, then the label-embedding gradient and the edge-encoder gradients of
@@ -1018,9 +815,8 @@ int bio_backward_tail(int type, const SideCtx* sc, const float* gT, const float*
   return PGNN_OK;
 }
 
-int bio_gin_forward(const void* const* params, void* const* bn_running_mean, void* const* bn_running_var, void* const* bn_num_batches_tracked,
-                    int64_t N, int64_t L, int64_t D, int training, float momentum, float eps, const Drops& drops, int precision,
-                    float* node_rep, int64_t ld_out, const BioGinWs& w, cudaStream_t st) {
+int bio_gin_forward(const void* const* params, const BnRun& bn, int64_t N, int64_t L, int64_t D, int training, const Drops& drops,
+                    int precision, float* node_rep, int64_t ld_out, const BioGinWs& w, cudaStream_t st) {
   const int64_t D2 = 2 * D;
   for (int64_t l = 0; l < L; ++l) {
     const void* const* p = params + PB_LAYER0 + l * BG_COUNT;
@@ -1037,33 +833,19 @@ int bio_gin_forward(const void* const* params, void* const* bn_running_mean, voi
     // Linear 1; on the tensor path in training its epilogue also accumulates the inner BatchNorm's batch statistics
     const float* gamma = (const float*)p[BG_GAMMA];
     const float* beta = (const float*)p[BG_BETA];
-    float* rm = (float*)bn_running_mean[l];
-    float* rv = (float*)bn_running_var[l];
-    int64_t* nbt = bn_num_batches_tracked ? (int64_t*)bn_num_batches_tracked[l] : nullptr;
     double* acc = w.bn_acc + l * 2 * D2;
-    bool stats_fused = false;
-    if (training && precision == 1) {
-      PGNN_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * 2 * D2, st));
-      PgnnGemmHooks hk;
-      hk.stats = acc;
-      const int rc = pgnn_tc_linear_fwd(aggr, D2, (const float*)p[BG_W1], (const float*)p[BG_B1], N, D2, D2, 0, z1, D2, st, &hk);
-      if (rc == PGNN_OK) stats_fused = true;
-      else if (rc != PGNN_EUNSUPPORTED) return rc;
-    }
-    if (!stats_fused) TRY(pgnn_linear_fwd(aggr, D2, (const float*)p[BG_W1], (const float*)p[BG_B1], N, D2, D2, 0, z1, D2, precision, st));
+    bool stats_fused;
+    TRY(linear_bn_stats(training ? acc : nullptr, Img{}, aggr, D2, (const float*)p[BG_W1], (const float*)p[BG_B1], N, D2, D2, z1, D2,
+                        precision, st, stats_fused));
     // inner BatchNorm1d(2D) + ReLU
     if (stats_fused) {
-      PgnnBnFold fold{};
-      fold.acc = acc; fold.gamma = gamma; fold.beta = beta;
-      fold.running_mean = rm; fold.running_var = rv; fold.nbt = nbt;
-      fold.save_mean = w.mean + l * D2; fold.save_invstd = w.invstd + l * D2;
-      fold.momentum = momentum; fold.eps = eps; fold.set_rows((int)N);
+      const PgnnBnFold fold = bn_fold(bn, l, acc, gamma, beta, w.mean + l * D2, w.invstd + l * D2, N);
       TRY(pgnn_internal_bn_apply_fold(z1, D2, N, D2, fold, 1, y1, D2, st, nullptr));
     } else if (training) {
-      TRY(pgnn_internal_bn_fwd_train(z1, D2, N, D2, gamma, beta, rm, rv, nbt, momentum, eps, 1, y1, D2, w.mean + l * D2, w.invstd + l * D2,
-                                     nullptr, nullptr, w.scratch, w.scratch_bytes, st, nullptr));
+      TRY(pgnn_internal_bn_fwd_train(z1, D2, N, D2, gamma, beta, bn.rm(l), bn.rv(l), bn.nb(l), bn.momentum, bn.eps, 1, y1, D2,
+                                     w.mean + l * D2, w.invstd + l * D2, nullptr, nullptr, w.scratch, w.scratch_bytes, st, nullptr));
     } else {
-      TRY(pgnn_bn_fwd_eval(z1, D2, N, D2, gamma, beta, rm, rv, eps, 1, y1, D2, st));
+      TRY(pgnn_bn_fwd_eval(z1, D2, N, D2, gamma, beta, bn.rm(l), bn.rv(l), bn.eps, 1, y1, D2, st));
     }
     // Linear 2: the layer's pre-activation; the last layer without dropout writes node_rep itself
     const bool direct = last && drop_out.p == 0.f;
@@ -1092,7 +874,7 @@ int bio_gin_backward(const void* const* params, const float* g_node_rep, int64_t
     float* gz2 = w.gz2 + (sc ? par * N * D : 0);
     float* gz1 = w.gz1 + (sc ? par * N * D2 : 0);
     // the gradient at the layer's pre-activation: its ReLU (inner layers) and dropout masks in one sweep
-    if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad has finished reading this copy
+    TRY(side_wait(sc, st, 0, par));
     const float* gz;
     int64_t ldgz;
     TRY(bio_act_bwd(gz, ldgz, gy, ldgy, w.z2 + l * N * D, N, D, last, drops.at(l), gz2, st));
@@ -1100,7 +882,7 @@ int bio_gin_backward(const void* const* params, const float* g_node_rep, int64_t
     TRY(side_wgrad(sc, st, 0, par, precision, gz, ldgz, y1, D2, N, D, D2, grads + o[BG_W2], grads + o[BG_B2], w.wpart, w.wpart_floats));
     TRY(pgnn_linear_bwd_x(gz, ldgz, (const float*)p[BG_W2], N, D, D2, nullptr, 0, w.gy1, D2, precision, st));
     // inner BatchNorm + ReLU (mask recomputed from z1); the same pass leaves colsum(gz1) = the gradient of mlp.0.bias
-    if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[1][par], 0));
+    TRY(side_wait(sc, st, 1, par));
     TRY(pgnn_internal_bn_bwd(w.gy1, D2, z1, D2, N, D2, (const float*)p[BG_GAMMA], (const float*)p[BG_BETA], w.mean + l * D2,
                              w.invstd + l * D2, 1, gz1, D2, grads + o[BG_GAMMA], grads + o[BG_BETA], grads + o[BG_B1], w.scratch,
                              w.scratch_bytes, st, nullptr));
@@ -1116,72 +898,130 @@ int bio_gin_backward(const void* const* params, const float* g_node_rep, int64_t
   return bio_backward_tail(kGin, sc, w.gT, w.gh, x, N, L, D, grads, off, st);
 }
 
-int bio_conv_forward(int type, const void* const* params, const float* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D,
-                     const Drops& drops, int precision, float* node_rep, int64_t ld_out, const BioConvWs& w, cudaStream_t st) {
+// ==============================================================================================================================
+// GCN / GraphSAGE / GAT, both domains
+// ==============================================================================================================================
+
+// A conv layer's edge term.  The gathers read the summary S [N, Q] against the table T (rows < q_split) and T2 (the rest); GAT
+// reads the one table T per edge, from the raw edge_attr as is_bio says.  The backward lands the table gradient on gT / gT2,
+// zeroing them first when zero_gT (GAT's backward overwrites its own).
+struct EdgeTerm {
+  const float* S;
+  int Q, q_split;
+  const float *T, *T2;
+  int is_bio;
+  float *gT, *gT2;
+  bool zero_gT;
+};
+
+// chem: the two bond tables (GAT: both in layer l's [9, C] workspace table, which the forward fills) and their gradients in the
+// flat buffer; bio: layer l's packed [10, C] table and its gradient, zeroed once per pass and unpacked by bio_backward_tail
+EdgeTerm edge_term(bool bio, int type, const ConvWs& w, const void* const* p, int64_t l, int64_t C, float* grads, const int64_t* o) {
+  if (bio) return EdgeTerm{w.S, kBioQ, kBioQ, w.T + l * kBioQ * C, nullptr, 1, w.gT + l * kBioQ * C, nullptr, false};
+  const int et = type == PGNN_CONV_GAT ? A_ET1 : G_ET1;
+  return EdgeTerm{w.S, kChemQ, kChemQSplit, type == PGNN_CONV_GAT ? w.T + l * kChemQ * C : (const float*)p[et], (const float*)p[et + 1], 0,
+                  grads ? grads + o[et] : nullptr, grads ? grads + o[et + 1] : nullptr, true};
+}
+
+// Every layer of a forward: Linear -> GAT | GCN gather | mean gather + L2 normalisation, then chem's BatchNorm (train or eval;
+// its apply takes the ReLU and dropout) or bio's ReLU + dropout sweep.
+int conv_forward(bool bio, int type, const void* const* params, const BnRun& bn, const void* edge_attr, int64_t N, int64_t E, int64_t L,
+                 int64_t D, int training, const Drops& drops, int precision, float* node_rep, int64_t ld_out, const ConvWs& w,
+                 cudaStream_t st) {
   const bool gat = type == PGNN_CONV_GAT;
-  const int64_t C = bio_width(type, D);
-  const int PL = bio_layer_params(type);
+  const int64_t C = gat ? kHeads * D : D;
+  const int PL = bio ? bio_layer_params(type) : layer_params(type);
   const float* h = w.h0;
   for (int64_t l = 0; l < L; ++l) {
-    const void* const* p = params + PB_LAYER0 + l * PL;
+    const void* const* p = params + (bio ? PB_LAYER0 : P_LAYER0) + l * PL;
     const bool last = l == L - 1;
     const PgnnDropout drop = drops.at(l);
+    const EdgeTerm e = edge_term(bio, type, w, p, l, C, nullptr, nullptr);
     float* xl = w.xl + l * N * C;
     float* z = w.z + l * N * D;
-    const float* T = w.T + l * kBioQ * C;
-    // the last layer without dropout writes node_rep itself, except GraphSAGE, whose backward reads its normalised rows
-    const bool direct = last && drop.p == 0.f && type != PGNN_CONV_SAGE && ld_out % 4 == 0 && aligned16(node_rep);
+    // bio: the last layer without dropout writes node_rep itself, except GraphSAGE, whose backward reads its normalised rows from z
+    const bool direct = bio && last && drop.p == 0.f && type != PGNN_CONV_SAGE && ld_out % 4 == 0 && aligned16(node_rep);
     float* out = direct ? node_rep : z;
     const int64_t ldo = direct ? ld_out : D;
-    TRY(pgnn_linear_fwd(h, D, (const float*)p[gat ? BA_W : BC_W], (const float*)p[gat ? BA_B : BC_B], N, C, D, 0, xl, C, precision, st));
+    TRY(pgnn_linear_fwd(h, D, (const float*)p[CV_W], (const float*)p[CV_B], N, C, D, 0, xl, C, precision, st));
     if (gat) {
-      TRY(pgnn_gat_fwd(xl, N, kHeads, D, (const float*)p[BA_ATT], T, 1, edge_attr, w.rowptr_t, w.nbr_t, w.eid_t, E, (const float*)p[BA_BIAS],
-                       kSlope, w.alpha + l * (E + N) * kHeads, w.pq + l * N * kHeads * 2, out, ldo, st));
+      if (!bio) {  // the kernels index one [9, H*D] table: rows 0..5 bond type, 6..8 bond direction
+        float* T = w.T + l * kChemQ * C;
+        PGNN_CUDA(cudaMemcpyAsync(T, p[A_ET1], sizeof(float) * 6 * C, cudaMemcpyDeviceToDevice, st));
+        PGNN_CUDA(cudaMemcpyAsync(T + 6 * C, p[A_ET2], sizeof(float) * 3 * C, cudaMemcpyDeviceToDevice, st));
+      }
+      TRY(pgnn_gat_fwd(xl, N, kHeads, D, (const float*)p[CV_ATT], e.T, e.is_bio, edge_attr, w.rowptr_t, w.nbr_t, w.eid_t, E,
+                       (const float*)p[CV_BIAS], kSlope, w.alpha + l * (E + N) * kHeads, w.pq + l * N * kHeads * 2, out, ldo, st));
     } else if (type == PGNN_CONV_GCN) {
-      TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_GCN, w.dinv, w.S, kBioQ, T, nullptr,
-                                      kBioQ, 0, out, ldo, st, nullptr, nullptr));
+      TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_GCN, w.dinv, e.S, e.Q, e.T, e.T2,
+                                      e.q_split, 0, out, ldo, st, nullptr, nullptr));
     } else {
       // mean aggregation into the backward scratch `gz` (only its normalised rows and their norms are needed later)
-      TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_MEAN, nullptr, w.S, kBioQ, T, nullptr,
-                                      kBioQ, 0, w.gz, D, st, nullptr, nullptr));
+      TRY(pgnn_internal_aggregate_fwd(xl, D, nullptr, nullptr, 0, N, D, w.rowptr_t, w.nbr_t, PGNN_AGG_MEAN, nullptr, e.S, e.Q, e.T, e.T2,
+                                      e.q_split, 0, w.gz, D, st, nullptr, nullptr));
       TRY(pgnn_l2norm_fwd(w.gz, D, N, D, z, D, w.nrm + l * N, st));
     }
     float* hout = w.hout + l * N * D;
-    if (!last) TRY(bio_act(false, z, D, nullptr, 0, N, D, 1, drop, hout, D, st));
-    else if (!direct) TRY(bio_act(false, z, D, nullptr, 0, N, D, 0, drop, node_rep, ld_out, st));
+    if (bio) {
+      if (!last) TRY(bio_act(false, z, D, nullptr, 0, N, D, 1, drop, hout, D, st));
+      else if (!direct) TRY(bio_act(false, z, D, nullptr, 0, N, D, 0, drop, node_rep, ld_out, st));
+    } else {
+      if (last) hout = node_rep;
+      const int64_t ldh = last ? ld_out : D;
+      const float* gamma = (const float*)p[gat ? A_GAMMA : G_GAMMA];
+      const float* beta = (const float*)p[gat ? A_BETA : G_BETA];
+      if (training) {
+        // after the ReLU: hout is the next layer's input and its Linear's weight-gradient operand
+        TRY(pgnn_internal_bn_fwd_train(z, D, N, D, gamma, beta, bn.rm(l), bn.rv(l), bn.nb(l), bn.momentum, bn.eps, !last, hout, ldh,
+                                       w.mean + l * D, w.invstd + l * D, nullptr, nullptr, w.scratch, w.scratch_bytes, st, &drop));
+      } else {
+        TRY(pgnn_bn_fwd_eval(z, D, N, D, gamma, beta, bn.rm(l), bn.rv(l), bn.eps, !last, hout, ldh, st));
+      }
+    }
     h = hout;
   }
   return PGNN_OK;
 }
 
-int bio_conv_backward(int type, const void* const* params, const float* g_node_rep, int64_t ldg, const float* x, const float* edge_attr,
-                      int64_t N, int64_t E, int64_t L, int64_t D, const Drops& drops, int precision, float* grads, const int64_t* off,
-                      const BioConvWs& w, cudaStream_t st) {
+// Every layer of a backward: the gradient at the conv's output (chem: BatchNorm backward; bio: the ReLU + dropout sweep), then
+// GAT backward | L2-normalisation backward + edge-table gradient + transpose gather, the Linear's weight gradient on the side
+// stream and its input gradient.  x is chem's int64 atom codes or bio's float labels.
+int conv_backward(bool bio, int type, const void* const* params, const float* g_node_rep, int64_t ldg, const void* x,
+                  const void* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, const Drops& drops, int precision, float* grads,
+                  const int64_t* off, const ConvWs& w, cudaStream_t st) {
   const bool gat = type == PGNN_CONV_GAT;
-  const int64_t C = bio_width(type, D);
-  const int PL = bio_layer_params(type);
+  const int64_t C = gat ? kHeads * D : D;
+  const int PL = bio ? bio_layer_params(type) : layer_params(type);
+  const int layer0 = bio ? PB_LAYER0 : P_LAYER0;
   SideCtx* sc = precision == 1 ? side_ctx(st) : nullptr;
-  if (!gat) PGNN_CUDA(cudaMemsetAsync(w.gT, 0, sizeof(float) * L * kBioQ * C, st));  // GAT's backward overwrites its table gradient
+  if (bio && !gat) PGNN_CUDA(cudaMemsetAsync(w.gT, 0, sizeof(float) * L * kBioQ * C, st));
   const float* gy = g_node_rep;
   int64_t ldgy = ldg;
   for (int64_t l = L - 1; l >= 0; --l) {
-    const void* const* p = params + PB_LAYER0 + l * PL;
-    const int64_t* o = off + PB_LAYER0 + l * PL;
+    const void* const* p = params + layer0 + l * PL;
+    const int64_t* o = off + layer0 + l * PL;
     const bool last = l == L - 1;
     const int par = (int)(l & 1);
     const float* xl = w.xl + l * N * C;
     const float* z = w.z + l * N * D;
     const float* hin = l == 0 ? w.h0 : w.hout + (l - 1) * N * D;
     float* gxl = w.gxl + (sc ? par * N * C : 0);
-    float* gT = w.gT + l * kBioQ * C;
-    const float* gz;
-    int64_t ldgz;
-    TRY(bio_act_bwd(gz, ldgz, gy, ldgy, z, N, D, last, drops.at(l), w.gz, st));
-    if (sc) PGNN_CUDA(cudaStreamWaitEvent(st, sc->done[0][par], 0));  // layer l+2's wgrad has finished reading this copy of gxl
+    const EdgeTerm e = edge_term(bio, type, w, p, l, C, grads, o);
+    const PgnnDropout drop = drops.at(l);
+    const float* gz = w.gz;
+    int64_t ldgz = D;
+    if (bio) {
+      TRY(bio_act_bwd(gz, ldgz, gy, ldgy, z, N, D, last, drop, w.gz, st));
+    } else {
+      const int g = gat ? A_GAMMA : G_GAMMA, b = gat ? A_BETA : G_BETA;
+      TRY(pgnn_internal_bn_bwd(gy, ldgy, z, D, N, D, (const float*)p[g], (const float*)p[b], w.mean + l * D, w.invstd + l * D, !last,
+                               w.gz, D, grads + o[g], grads + o[b], nullptr, w.scratch, w.scratch_bytes, st, &drop));
+    }
+    TRY(side_wait(sc, st, 0, par));
     if (gat) {
-      TRY(pgnn_gat_bwd(gz, ldgz, xl, N, kHeads, D, (const float*)p[BA_ATT], w.T + l * kBioQ * C, 1, edge_attr, w.rowptr_t, w.nbr_t, w.eid_t,
+      TRY(pgnn_gat_bwd(gz, ldgz, xl, N, kHeads, D, (const float*)p[CV_ATT], e.T, e.is_bio, edge_attr, w.rowptr_t, w.nbr_t, w.eid_t,
                        w.rowptr_s, w.nbr_s, w.eid_s, E, kSlope, w.alpha + l * (E + N) * kHeads, w.pq + l * N * kHeads * 2, gxl,
-                       grads + o[BA_ATT], gT, grads + o[BA_BIAS], w.scratch, w.scratch_bytes, st));
+                       grads + o[CV_ATT], e.gT, grads + o[CV_BIAS], w.scratch, w.scratch_bytes, st));
     } else {
       const float* ga = gz;
       int64_t ldga = ldgz;
@@ -1190,17 +1030,45 @@ int bio_conv_backward(int type, const void* const* params, const float* g_node_r
         ga = w.ga;
         ldga = D;
       }
-      TRY(pgnn_internal_edge_table_bwd2(w.S, kBioQ, ga, ldga, 0, N, (int)D, gT, D, nullptr, kBioQ, st));
+      if (e.zero_gT) PGNN_CUDA(cudaMemsetAsync(e.gT, 0, sizeof(float) * e.Q * C, st));  // chem: the two tables are adjacent
+      TRY(pgnn_internal_edge_table_bwd2(e.S, e.Q, ga, ldga, 0, N, (int)D, e.gT, D, e.gT2, e.q_split, st));
       TRY(pgnn_aggregate_bwd(ga, ldga, N, D, w.rowptr_s, w.nbr_s, agg_mode(type), w.dinv, w.rowptr_t, gxl, D, st));
     }
     // Linear: weight + bias gradients (side stream), then the input gradient
-    TRY(side_wgrad(sc, st, 0, par, precision, gxl, C, hin, D, N, C, D, grads + o[gat ? BA_W : BC_W], grads + o[gat ? BA_B : BC_B], w.wpart,
-                   w.wpart_floats));
-    TRY(pgnn_linear_bwd_x(gxl, C, (const float*)p[gat ? BA_W : BC_W], N, C, D, nullptr, 0, w.gh, D, precision, st));
+    TRY(side_wgrad(sc, st, 0, par, precision, gxl, C, hin, D, N, C, D, grads + o[CV_W], grads + o[CV_B], w.wpart, w.wpart_floats));
+    TRY(pgnn_linear_bwd_x(gxl, C, (const float*)p[CV_W], N, C, D, nullptr, 0, w.gh, D, precision, st));
     gy = w.gh;
     ldgy = D;
   }
-  return bio_backward_tail(type, sc, w.gT, w.gh, x, N, L, D, grads, off, st);
+  if (bio) return bio_backward_tail(type, sc, w.gT, w.gh, (const float*)x, N, L, D, grads, off, st);
+  return embed_backward(sc, w, w.gh, (const int64_t*)x, N, D, precision, grads, off, w.wpart, w.wpart_floats, st);
+}
+
+int64_t workspace_bytes(bool bio, int type, int64_t N, int64_t E, int64_t L, int64_t D) {
+  if (type != kGin) return carve_conv(nullptr, bio, type, N, E, L, D).total;
+  return bio ? carve_bio_gin(nullptr, N, E, L, D).total : carve_gin(nullptr, N, E, L, D).total;
+}
+
+// The start of every pass of either domain, in this order: the checks both passes share plus `ok` (the pass's own), the
+// workspace size, then N == 0, which ends the call (run = false; a backward zeroes its gradients).  A backward (off != nullptr)
+// gets its flat gradient layout.
+int begin_pass(bool bio, int type, float drop_p, bool ok, int64_t N, int64_t E, int64_t L, int64_t D, const void* params,
+               void* workspace, int64_t workspace_size, float* grads, std::vector<int64_t>* off, cudaStream_t st, bool& run) {
+  run = false;
+  PGNN_CHECK_ARG(valid_type(type) && drop_p >= 0.f && drop_p <= 1.f && ok);
+  PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && workspace);
+  if (workspace_size < workspace_bytes(bio, type, N, E, L, D)) return PGNN_EWORKSPACE;
+  if (off) {
+    off->resize((bio ? bio_grad_layout(type, L, D, nullptr) : grad_layout(type, L, D, nullptr)) + 1);
+    if (bio) bio_grad_layout(type, L, D, off->data());
+    else grad_layout(type, L, D, off->data());
+  }
+  if (N == 0) {
+    if (off) PGNN_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * off->back(), st));
+    return PGNN_OK;
+  }
+  run = true;
+  return PGNN_OK;
 }
 
 }  // namespace
@@ -1220,7 +1088,7 @@ int pgnn_chem_gin_grad_offsets(int64_t L, int64_t D, int64_t* offsets /*host [nu
 
 int64_t pgnn_chem_gin_workspace_bytes(int64_t N, int64_t E, int64_t L, int64_t D) {
   if (N < 0 || E < 0 || L < 1 || D <= 0) return PGNN_EINVAL;
-  return carve_gin(nullptr, N, E, L, D).total;
+  return workspace_bytes(false, kGin, N, E, L, D);
 }
 
 int pgnn_chem_gin_forward(const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
@@ -1277,7 +1145,7 @@ int pgnn_chem_conv_grad_offsets(int conv_type, int64_t L, int64_t D, int64_t* of
 
 int64_t pgnn_chem_conv_workspace_bytes(int conv_type, int64_t N, int64_t E, int64_t L, int64_t D) {
   if (!valid_conv(conv_type) || N < 0 || E < 0 || L < 1 || D <= 0) return PGNN_EINVAL;
-  return carve_conv(nullptr, conv_type, N, E, L, D).total;
+  return workspace_bytes(false, conv_type, N, E, L, D);
 }
 
 int pgnn_chem_conv_forward(int conv_type, const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
@@ -1305,25 +1173,39 @@ int pgnn_chem_encoder_forward(int gnn_type, const void* const* params, void* con
                               int64_t N, int64_t E, int64_t L, int64_t D, int training, float momentum, float eps, float drop_p,
                               int64_t drop_seed, int precision, float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes,
                               void* stream) {
-  PGNN_CHECK_ARG((gnn_type == kGin || valid_conv(gnn_type)) && drop_p >= 0.f && drop_p <= 1.f);
+  cudaStream_t st = as_stream(stream);
+  bool run;
+  TRY(begin_pass(false, gnn_type, drop_p,
+                 bn_running_mean && bn_running_var && (N == 0 || (x && node_rep)) && (gnn_type == kGin || E == 0 || (edge_index && edge_attr)),
+                 N, E, L, D, params, workspace, workspace_bytes, nullptr, nullptr, st, run));
+  if (!run) return PGNN_OK;
   Drops drops;
   if (training) drops = Drops{drop_p, drop_seed};  // eval mode has no dropout
-  if (gnn_type == kGin)
-    return gin_forward(params, bn_running_mean, bn_running_var, bn_num_batches_tracked, x, edge_index, edge_attr, N, E, L, D, training, momentum,
-                       eps, drops, precision, node_rep, ld_out, workspace, workspace_bytes, stream);
-  return conv_forward(gnn_type, params, bn_running_mean, bn_running_var, bn_num_batches_tracked, x, edge_index, edge_attr, N, E, L, D, training,
-                      momentum, eps, drops, precision, node_rep, ld_out, workspace, workspace_bytes, stream);
+  const BnRun bn{bn_running_mean, bn_running_var, bn_num_batches_tracked, momentum, eps};
+  if (gnn_type == kGin) {
+    const GinWs w = carve_gin(workspace, N, E, L, D);
+    TRY(forward_prologue(kGin, w, params, x, edge_index, edge_attr, N, E, D, training, precision, w.scratch, w.scratch_bytes, st));
+    return gin_forward(params, bn, training, drops, precision, node_rep, ld_out, N, L, D, w, st);
+  }
+  const ConvWs w = carve_conv(workspace, false, gnn_type, N, E, L, D);
+  TRY(forward_prologue(gnn_type, w, params, x, edge_index, edge_attr, N, E, D, training, precision, w.scratch, w.scratch_bytes, st));
+  return conv_forward(false, gnn_type, params, bn, edge_attr, N, E, L, D, training, drops, precision, node_rep, ld_out, w, st);
 }
 
 int pgnn_chem_encoder_backward(int gnn_type, const void* const* params, const float* g_node_rep, int64_t ldg, const int64_t* x,
                                const int64_t* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, float drop_p, int64_t drop_seed,
                                int precision, float* grads, void* workspace, int64_t workspace_bytes, void* stream) {
-  PGNN_CHECK_ARG((gnn_type == kGin || valid_conv(gnn_type)) && drop_p >= 0.f && drop_p <= 1.f);
+  cudaStream_t st = as_stream(stream);
+  std::vector<int64_t> off;
+  bool run;
+  TRY(begin_pass(false, gnn_type, drop_p, grads != nullptr, N, E, L, D, params, workspace, workspace_bytes, grads, &off, st, run));
+  if (!run) return PGNN_OK;
+  PGNN_CHECK_ARG(g_node_rep && x && (gnn_type == kGin || E == 0 || edge_attr));
   const Drops drops{drop_p, drop_seed};
   if (gnn_type == kGin)
-    return gin_backward(params, g_node_rep, ldg, x, N, E, L, D, drops, precision, grads, workspace, workspace_bytes, stream);
-  return conv_backward(gnn_type, params, g_node_rep, ldg, x, edge_attr, N, E, L, D, drops, precision, grads, workspace, workspace_bytes,
-                       stream);
+    return gin_backward(params, g_node_rep, ldg, x, N, L, D, drops, precision, grads, off.data(), carve_gin(workspace, N, E, L, D), st);
+  return conv_backward(false, gnn_type, params, g_node_rep, ldg, x, edge_attr, N, E, L, D, drops, precision, grads, off.data(),
+                       carve_conv(workspace, false, gnn_type, N, E, L, D), st);
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------
@@ -1342,7 +1224,7 @@ int pgnn_bio_encoder_grad_offsets(int gnn_type, int64_t L, int64_t D, int64_t* o
 
 int64_t pgnn_bio_encoder_workspace_bytes(int gnn_type, int64_t N, int64_t E, int64_t L, int64_t D) {
   if (!valid_type(gnn_type) || N < 0 || E < 0 || L < 1 || D <= 0) return PGNN_EINVAL;
-  return bio_workspace_bytes(gnn_type, N, E, L, D);
+  return workspace_bytes(true, gnn_type, N, E, L, D);
 }
 
 int pgnn_bio_encoder_forward(int gnn_type, const void* const* params, void* const* bn_running_mean, void* const* bn_running_var,
@@ -1350,48 +1232,41 @@ int pgnn_bio_encoder_forward(int gnn_type, const void* const* params, void* cons
                              int64_t N, int64_t E, int64_t L, int64_t D, int training, float momentum, float eps, float drop_p,
                              int64_t drop_seed, int precision, float* node_rep, int64_t ld_out, void* workspace, int64_t workspace_bytes,
                              void* stream) {
-  PGNN_CHECK_ARG(valid_type(gnn_type) && drop_p >= 0.f && drop_p <= 1.f);
-  PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && workspace);
-  PGNN_CHECK_ARG(gnn_type != kGin || (bn_running_mean && bn_running_var));
-  PGNN_CHECK_ARG(N == 0 || (x && node_rep && ld_out >= D));
-  PGNN_CHECK_ARG(E == 0 || (edge_index && edge_attr));
-  if (workspace_bytes < bio_workspace_bytes(gnn_type, N, E, L, D)) return PGNN_EWORKSPACE;
-  if (N == 0) return PGNN_OK;
+  cudaStream_t st = as_stream(stream);
+  bool run;
+  TRY(begin_pass(true, gnn_type, drop_p,
+                 (gnn_type != kGin || (bn_running_mean && bn_running_var)) && (N == 0 || (x && node_rep && ld_out >= D)) &&
+                     (E == 0 || (edge_index && edge_attr)),
+                 N, E, L, D, params, workspace, workspace_bytes, nullptr, nullptr, st, run));
+  if (!run) return PGNN_OK;
   Drops drops;
   if (training) drops = Drops{drop_p, drop_seed};  // eval mode has no dropout
-  cudaStream_t st = as_stream(stream);
+  const BnRun bn{bn_running_mean, bn_running_var, bn_num_batches_tracked, momentum, eps};
   if (gnn_type == kGin) {
     const BioGinWs w = carve_bio_gin(workspace, N, E, L, D);
     TRY(bio_prologue(kGin, w, w.T, params, x, edge_index, edge_attr, N, E, L, D, w.scratch, w.scratch_bytes, st));
-    return bio_gin_forward(params, bn_running_mean, bn_running_var, bn_num_batches_tracked, N, L, D, training, momentum, eps, drops,
-                           precision, node_rep, ld_out, w, st);
+    return bio_gin_forward(params, bn, N, L, D, training, drops, precision, node_rep, ld_out, w, st);
   }
-  const BioConvWs w = carve_bio_conv(workspace, gnn_type, N, E, L, D);
+  const ConvWs w = carve_conv(workspace, true, gnn_type, N, E, L, D);
   TRY(bio_prologue(gnn_type, w, w.T, params, x, edge_index, edge_attr, N, E, L, D, w.scratch, w.scratch_bytes, st));
-  return bio_conv_forward(gnn_type, params, edge_attr, N, E, L, D, drops, precision, node_rep, ld_out, w, st);
+  return conv_forward(true, gnn_type, params, bn, edge_attr, N, E, L, D, training, drops, precision, node_rep, ld_out, w, st);
 }
 
 int pgnn_bio_encoder_backward(int gnn_type, const void* const* params, const float* g_node_rep, int64_t ldg, const float* x,
                               const float* edge_attr, int64_t N, int64_t E, int64_t L, int64_t D, float drop_p, int64_t drop_seed,
                               int precision, float* grads, void* workspace, int64_t workspace_bytes, void* stream) {
-  PGNN_CHECK_ARG(valid_type(gnn_type) && drop_p >= 0.f && drop_p <= 1.f);
-  PGNN_CHECK_ARG(N >= 0 && E >= 0 && L >= 1 && D > 0 && D % 4 == 0 && params && grads && workspace);
-  if (workspace_bytes < bio_workspace_bytes(gnn_type, N, E, L, D)) return PGNN_EWORKSPACE;
-  const int64_t count = bio_grad_layout(gnn_type, L, D, nullptr);
-  std::vector<int64_t> offsets(count + 1);
-  bio_grad_layout(gnn_type, L, D, offsets.data());
   cudaStream_t st = as_stream(stream);
-  if (N == 0) {
-    PGNN_CUDA(cudaMemsetAsync(grads, 0, sizeof(float) * offsets[count], st));
-    return PGNN_OK;
-  }
+  std::vector<int64_t> off;
+  bool run;
+  TRY(begin_pass(true, gnn_type, drop_p, grads != nullptr, N, E, L, D, params, workspace, workspace_bytes, grads, &off, st, run));
+  if (!run) return PGNN_OK;
   PGNN_CHECK_ARG(g_node_rep && x && ldg >= D && (E == 0 || gnn_type != PGNN_CONV_GAT || edge_attr));
   const Drops drops{drop_p, drop_seed};
   if (gnn_type == kGin)
-    return bio_gin_backward(params, g_node_rep, ldg, x, N, L, D, drops, precision, grads, offsets.data(),
-                            carve_bio_gin(workspace, N, E, L, D), st);
-  return bio_conv_backward(gnn_type, params, g_node_rep, ldg, x, edge_attr, N, E, L, D, drops, precision, grads, offsets.data(),
-                           carve_bio_conv(workspace, gnn_type, N, E, L, D), st);
+    return bio_gin_backward(params, g_node_rep, ldg, x, N, L, D, drops, precision, grads, off.data(), carve_bio_gin(workspace, N, E, L, D),
+                            st);
+  return conv_backward(true, gnn_type, params, g_node_rep, ldg, x, edge_attr, N, E, L, D, drops, precision, grads, off.data(),
+                       carve_conv(workspace, true, gnn_type, N, E, L, D), st);
 }
 
 }  // extern "C"
